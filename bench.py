@@ -46,17 +46,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
         except Exception:
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
-
-
-def ncu_traffic(kernel):
-    """DRAM bytes per frame of `kernel` from the committed `ncu --set full` capture
-    (profiles/ncu_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum)."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        return json.load(open(p)).get(kernel)
-    except Exception:
-        return None
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s of HBM3"
 
 
 class ClockSampler:
@@ -553,7 +543,10 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed steps of the headline and of the configs[1] / configs[3] legs (and, with "
+                         "--all-legs, of the device-timed secondary legs); the single-frame leg times 20 "
+                         "launches with L2 flushes between them, the host-buffer runs 3 or 5")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
     ap.add_argument("--total-frames", type=int, default=FRAMES_TOTAL,
@@ -578,6 +571,10 @@ def main():
     ap.add_argument("--unvalidated", action="store_true",
                     help="with --all-legs: include the post-decode kernels K9-K12 and Panasonic V4")
     ap.add_argument("--skip-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step decoded to DIR/<name>.npy "
+                         "(a fixed sample of every frame, two whole crops, per-segment results); with "
+                         "several GPUs, rank 0 writes its own shard: the first 256/N frames")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -639,6 +636,8 @@ def main():
         l0 = ctx.launches
         ms = time_steps(torch, run, args.steps, args.warmup, dist)
         launches = ctx.launches - l0 - args.warmup * plan.launches
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, torch, batch, d_out, plan.results())
         sus_n, sus_ms = 0, 0.0
         t_pre = time.perf_counter()
         while time.perf_counter() - t_pre < args.sustain_s:
@@ -663,10 +662,6 @@ def main():
                     "note": "in+out accounting of SURVEY 8(d): compressed bytes read once + 2 B/pixel written "
                             "once; read_only_frac = compressed bytes only (north_star's wording) -- the 2 B/pixel "
                             "of output cap it at ~0.34 when the in+out fraction is 1"}
-        tr = ncu_traffic(kern.split(" ")[0])
-        if tr:
-            roofline["traffic"] = tr["dram_bytes_per_frame"] * batch.n
-            roofline["traffic_source"] = tr["source"]
         sustained = None
         if sus_n:
             sp = sus_ms / sus_n
@@ -726,7 +721,7 @@ def main():
                            "frames_total": FT, "frames_per_gpu": per,
                            "bytes_per_step_per_gpu": in_b + out_b,
                            "compressed_bytes_per_pixel": in_b / pixels,
-                           "l2": "inputs+outputs of one step (%.1f GB per GPU) exceed the 126 MB L2; no flush needed"
+                           "l2": "inputs+outputs of one step (%.1f GB per GPU) exceed the 50 MB L2; no flush needed"
                                  % ((in_b + out_b) / 1e9),
                            "parallelism": "frames sharded across ranks (contiguous blocks of 256/N), no data-path "
                                           "collective in `value`; the NVLink output gather is `gather`",
@@ -744,6 +739,33 @@ def main():
     finally:
         shm.close()
         shm.unlink()
+
+
+DUMP_SAMPLES = 16384     # pixels per frame in pixels_sample.npy (same seeded positions in every frame)
+DUMP_SEED = 2024
+DUMP_CROP = (1024, 2048)  # rows x columns of the top-left crops of the first and the last frame
+
+
+def dump_outputs(out_dir, torch, batch, d_out, results):
+    """What the timed step returns to its caller, as float32 / float64 .npy files (about 35 MB for
+    the 256-frame batch): every frame's pixels at DUMP_SAMPLES seeded positions (the positions in
+    sample_yx.npy), whole crops of the first and the last frame, and per segment (tile) the status
+    and the bytes consumed that the plan reports."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(DUMP_SEED)
+    ys = rng.integers(0, H, DUMP_SAMPLES)
+    xs = rng.integers(0, W, DUMP_SAMPLES)
+    n, ob2, pitch2 = batch.n, batch.ob // 2, batch.out_pitch // 2
+    frames = d_out[:n * batch.ob].view(torch.int16).view(n, ob2)
+    idx = torch.from_numpy(ys * pitch2 + xs).cuda()
+    px = frames.index_select(1, idx).to(torch.int32) & 0xFFFF
+    np.save(os.path.join(out_dir, "pixels_sample.npy"), px.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "sample_yx.npy"), np.stack([ys, xs], axis=1).astype(np.float64))
+    ch, cw = DUMP_CROP
+    for name, k in (("frame_first_crop", 0), ("frame_last_crop", n - 1)):
+        img = frames[k, :H * pitch2].view(H, pitch2)[:ch, :cw].to(torch.int32) & 0xFFFF
+        np.save(os.path.join(out_dir, name + ".npy"), img.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "segment_results.npy"), np.asarray(results, dtype=np.float64).reshape(-1, 2))
 
 
 def kernel_name(plan, nframes):
@@ -787,9 +809,8 @@ def gpu_numa_cpus(local):
 
 def pin_rank_to_numa(local):
     """Keep this rank's threads, and therefore its pinned staging buffers (first touch), on the cores
-    of the NUMA node its GPU hangs off (sysfs; r2_run15: on a 4-GPU allocation GPUs 2 and 3 sit on
-    node 1).  Fallback when sysfs / nvidia-smi do not tell: GPUs 0-3 on node 0, 4-7 on node 1 (the
-    8-GPU boxes, SCALE_r01.json topology)."""
+    of the NUMA node its GPU hangs off (sysfs).  Fallback when sysfs / nvidia-smi do not tell:
+    GPUs 0-3 on node 0, 4-7 on node 1 (the usual topology of two-socket 8-GPU servers)."""
     try:
         ncpu = os.cpu_count() or 1
         if ncpu < 64 or not hasattr(os, "sched_setaffinity"):
@@ -835,8 +856,8 @@ def bench_gather_abi(torch, dist, rs, ctx, batch, world, rank, args, total_pixel
         for r in range(world):
             ok = ok and int(d_all[r * slab:r * slab + 1024 * 1024].to(torch.int64).sum().item()) == int(sums[r].item())
     out["gathered_matches_the_owners"] = bool(ok)
-    out["bound"] = ("the consumer GPU receives (N-1)/N of %.1f GB; at the 900 GB/s per direction of NVLink 5 that "
-                    "alone is %.1f ms" % (world * slab / 1e9, (world - 1) * slab / 900e9 * 1e3))
+    out["bound"] = ("the consumer GPU receives (N-1)/N of %.1f GB; at the 450 GB/s per direction of an H100's "
+                    "NVLink that alone is %.1f ms" % (world * slab / 1e9, (world - 1) * slab / 450e9 * 1e3))
     comm.close()
     del d_all
     return out
@@ -881,10 +902,6 @@ def bench_single_frame(torch, rs, ctx, port, synth, args, shm, cap, recs, peak, 
                         "frac": (in_b + out_b) / (ms * 1e-3) / 1e9 / peak,
                         "read_only_frac": in_b / (ms * 1e-3) / 1e9 / peak, "peak_source": peak_src,
                         "traffic": None}}
-    tr = ncu_traffic(ent["kernel"].split(" ")[0])
-    if tr:
-        ent["roofline"]["traffic"] = tr["dram_bytes_per_frame"]
-        ent["roofline"]["traffic_source"] = tr["source"]
     del flush
     # host buffers through the C ABI: pinned and pageable
     h_out = torch.empty(b1.out_bytes, dtype=torch.uint8, pin_memory=True)
@@ -940,7 +957,7 @@ def bench_core_others(torch, rs, ctx, port, synth, args, dist, peak):
     port.unpack(data, want, W, 1, (0, 0, W, H), pitch, BPS, port.MSB)
     got = d_out[:out_pitch * H].cpu().numpy().view(np.uint16).reshape(H, out_pitch // 2)
     exact = bool(np.array_equal(got[:, :W], want[:, :W]))
-    n = max(5, min(args.steps, 20))
+    n = args.steps
     ms = time_steps(torch, lambda: plan.run(d_in, d_out), n, 3, dist) / n
     in_b, out_b, pixels = plan.bytes()
     out["configs[1] 14-bit packed (MSB) unpack 8256x5504, %d frames per launch" % F] = {
@@ -966,7 +983,7 @@ def bench_core_others(torch, rs, ctx, port, synth, args, dist, peak):
     res = plan.results()
     got = d_out.cpu().numpy().view(np.uint16).reshape(cimg.shape)
     exact = bool(np.array_equal(got[:, :cw], cimg[:, :cw])) and res[0][0] == 0
-    ms = time_steps(torch, lambda: plan.run((d_in.data_ptr(), blob.size), d_out), 5, 2, dist) / 5
+    ms = time_steps(torch, lambda: plan.run((d_in.data_ptr(), blob.size), d_out), args.steps, 2, dist) / args.steps
     ent = {"MPixels/s": cw * ch / (ms * 1e-3) / 1e6, "ms_per_frame": ms, "bit_exact": exact,
            "kernels": "k2_range_count/verify/diffs + k3_column/row"}
     if not args.skip_cpu and int(os.environ.get("RANK", "0")) == 0:
@@ -992,7 +1009,7 @@ def bench_gather(torch, dist, d_out, world, rank, plan, d_in, args, frames, out_
         plan.run(d_in, d_out)
         # copy-free form: preallocated result, the collective's own layout (frame r + k*world at [r, k])
         shard.gather_frames(local, frames * world, dist, out=gathered, reorder=False)
-    n = max(2, min(args.steps, 5))
+    n = args.steps
     ms = time_steps(torch, step, n, 1, dist)
     total = frames * world * out_fb
     return {"what": "decode + ncclAllGather of the uint16 outputs over NVLink (all ranks get all frames)",
@@ -1007,7 +1024,7 @@ def bench_others(torch, rs, ctx, port, synth, args, dist, peak):
     if args.unvalidated and args.only_unvalidated:
         return bench_unvalidated(torch, rs, ctx, port, synth, args, dist, peak)
     out = {}
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     # ---- C3: 8256x5504 DNG, 726 LJPEG tiles of 256x256, 2 components ----
     img = synth.image_model(W, H, 12345)
     t = synth.make_dng_ljpeg(img, 256, 256)
@@ -1154,7 +1171,7 @@ def bench_others(torch, rs, ctx, port, synth, args, dist, peak):
 def bench_codecs(torch, rs, ctx, port, synth, args, dist, peak):
     """SURVEY 8(f)2/4: Canon sRaw interpolation, the Pentax PEF codec, Sony ARW2; device-timed."""
     out = {}
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     rank0 = int(os.environ.get("RANK", "0")) == 0
     # ---- Cr2sRawInterpolator, 4:2:0 version 2, 5040x3360 RGB output (mRAW class) ----
     num_mcus, rows = 2520, 1680
@@ -1440,7 +1457,7 @@ def bench_unvalidated(torch, rs, ctx, port, synth, args, dist, peak):
     """SURVEY 8(f)3 (+ Panasonic V4): kernels written after round 1's GPU budget was spent.  Off by
     default (--unvalidated); every leg first checks the result against the oracle."""
     out = {}
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     W, H = 8256, 5504
     pitch = rs.image_pitch(W)
     rng = np.random.default_rng(9)
@@ -1577,7 +1594,7 @@ def bench_forms(torch, rs, ctx, port, synth, args, dist, peak):
     frame each, device-timed like the headline (inputs resident in HBM)."""
     from rawspeed_b200 import formats as F
     out = {}
-    steps = max(3, min(args.steps, 10))
+    steps = args.steps
     cases = [("decode12BitRawWithControl<big>", F.RAW_12BIT_CONTROL_BE, 12 * W // 8 + (W + 2) // 10,
               port.FORM_12BIT_CONTROL_BE, 12, port.MSB, False),
              ("decode12BitRawUnpackedLeftAligned<little>", F.RAW_12BIT_LEFT_LE, 2 * W,

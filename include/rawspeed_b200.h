@@ -1,5 +1,5 @@
 /*
- * rawspeed_b200.h -- C ABI of the B200-native RAW decompression engine.
+ * rawspeed_b200.h -- C ABI of the H100-native RAW decompression engine.
  *
  * This is the drop-in boundary for rawspeed's per-pixel decode hot path.  The
  * reference (darktable-org/rawspeed) has no FFI layer; its seam is four C++

@@ -16,6 +16,7 @@ from . import port, synth  # noqa: F401
 try:  # the reference arm is optional (absent until `make -C oracle ref`)
     from . import ref  # noqa: F401
     HAVE_REF = ref.available()
+    REF_CHECKABLE = ref.checkable()   # built, or its results recorded under tests/golden/
 except OSError:  # pragma: no cover
     ref = None
-    HAVE_REF = False
+    HAVE_REF = REF_CHECKABLE = False

@@ -1,11 +1,11 @@
-"""rawspeed_b200 -- B200-native (sm_100a) RAW decompression engine for the
+"""rawspeed_b200 -- H100-native (sm_90a) RAW decompression engine for the
 per-pixel decode hot path of darktable-org/rawspeed.
 
     csrc/             hand-written CUDA kernels + the extern "C" ABI
                       (include/rawspeed_b200.h) + the C++ host mirror of the
                       reference's decompressor classes (csrc/host/)
     _abi.py / api.py  ctypes face of the ABI (plans, contexts)
-    build.py          in-tree nvcc build for sm_100a
+    build.py          in-tree nvcc build for sm_90a
 
 Nothing in this package imports oracle/ (the CPU checker).  There is no CPU
 fallback: without the CUDA library and a GPU the API raises."""

@@ -1,4 +1,4 @@
-"""Build the CUDA extension IN-TREE for sm_100a (B200).  nvcc cross-compiles
+"""Build the CUDA extension IN-TREE for sm_90a (H100).  nvcc cross-compiles
 without a GPU.  Produces rawspeed_b200/librawspeed_b200.so (the C-ABI library
 declared in include/rawspeed_b200.h) and rawspeed_b200/librawspeed_b200_host.so
 (the C++ host mirror of the reference's decompressor classes)."""
@@ -13,7 +13,7 @@ LIB = os.path.join(HERE, "librawspeed_b200.so")
 HOST_LIB = os.path.join(HERE, "librawspeed_b200_host.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
     "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fopenmp", "-shared",
 ]
 

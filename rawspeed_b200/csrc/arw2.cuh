@@ -1,4 +1,4 @@
-// arw2.cuh -- K6: Sony ARW2 block codec (SURVEY 8(f)4), sm_100a.
+// arw2.cuh -- K6: Sony ARW2 block codec (SURVEY 8(f)4), sm_90a.
 //
 // Replaces the body of SonyArw2Decompressor::decompressRow
 // (decompressors/SonyArw2Decompressor.cpp:58-112) and the per-row OpenMP loop

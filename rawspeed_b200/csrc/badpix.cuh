@@ -1,4 +1,4 @@
-// badpix.cuh -- K11: bad-pixel interpolation in place (sm_100a).
+// badpix.cuh -- K11: bad-pixel interpolation in place (sm_90a).
 // Reference: RawImageData::fixBadPixels / fixBadPixelsThread (common/RawImage.cpp:231-239,
 // :297-323) + RawImageDataU16::fixBadPixel (common/RawImageDataU16.cpp:399-485); the
 // per-pixel arithmetic is in badpix_core.h (shared with the CPU replay in tests/emu).
@@ -8,8 +8,7 @@
 // consults is the reference's mBadPixelMap.  Work is proportional to the number of bad
 // pixels, not to the image: a latency-bound scatter of a few thousand threads.
 //
-// Developed against a CPU replay of the thread program (tests/test_badpix_emu.py); first run on
-// a B200: bit-exact (profiles/r1_postdecode_first_gpu_run.md).
+// Developed against a CPU replay of the thread program (tests/test_badpix_emu.py).
 #pragma once
 
 #include "badpix_core.h"

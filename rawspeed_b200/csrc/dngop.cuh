@@ -1,4 +1,4 @@
-// dngop.cuh -- K10: a DNG opcode list applied to a decoded image in ONE pass, in place (sm_100a).
+// dngop.cuh -- K10: a DNG opcode list applied to a decoded image in ONE pass, in place (sm_90a).
 // Reference: DngOpcodes::applyOpCodes (common/DngOpcodes.cpp:730-735), one pass over the image
 // per opcode (:390-409); the per-sample arithmetic is in dngop_core.h (shared with the CPU
 // replay in tests/emu).
@@ -9,9 +9,8 @@
 // per sample regardless of the length of the list: HBM bound.  Lookup tables (128 KB each)
 // and delta arrays stay in L2.
 //
-// Developed against a CPU replay of the thread program (tests/test_dngop_emu.py); first run on
-// a B200: bit-exact (profiles/r1_postdecode_first_gpu_run.md), 0.51 ms per 45 MP frame with
-// eight opcodes -- issue bound (the per-sample lattice tests), the next thing to tune.
+// Developed against a CPU replay of the thread program (tests/test_dngop_emu.py); issue bound
+// (the per-sample lattice tests).
 #pragma once
 
 #include "common.cuh"

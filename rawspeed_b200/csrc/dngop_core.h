@@ -126,12 +126,11 @@ RSD_HD void dngop_apply_group_v1(const DngOpDev* ops, uint32_t nops, const uint1
   }
 }
 
-// ---- second version of the walk (the default since r2_run22; -DRSB200_DNGOP_V1 selects the first) ----
+// ---- second version of the walk (the default; -DRSB200_DNGOP_V1 selects the first) ----
 // The first version pays, per opcode and SAMPLE, a division by the run-time column pitch and a
 // switch on the opcode kind.  Here the lattice position of the group's first column is computed
 // once per opcode (one division) and stepped incrementally as the column advances, and the
-// kind is dispatched once per opcode, outside the sample loop.  First measured on a B200 the
-// first version was issue bound (0.51 ms per 45 MP frame with eight opcodes); this one: 0.47 ms.
+// kind is dispatched once per opcode, outside the sample loop (the first version is issue bound).
 template <class Sink>
 RSD_HD void dngop_apply_group_v2(const DngOpDev* ops, uint32_t nops, const uint16_t* tables,
                                  const uint32_t* deltas, const DngOpJobDev& jb, uint32_t r,
@@ -227,7 +226,7 @@ RSD_HD void dngop_apply_group_v2(const DngOpDev* ops, uint32_t nops, const uint1
 }
 
 // ---- third version of the walk: one sample per pixel (cpp = 1, every CFA image) ----
-// ncu on the second version (r2_postdecode_ncu_metrics.csv): issue bound at ~300 thread-instructions
+// The second version is issue bound at ~300 thread-instructions
 // per opcode and group -- eight rounds of range / lattice / plane tests, eight delta indices, and
 // twelve scalar loads of the opcode.  With one sample per pixel the eight samples of a group are
 // eight consecutive columns, so the opcode's footprint in the group is a bit mask with a closed
@@ -337,7 +336,6 @@ template <class Sink>
 RSD_HD void dngop_apply_group(const DngOpDev* ops, uint32_t nops, const uint16_t* tables,
                               const uint32_t* deltas, const DngOpJobDev& jb, uint32_t r,
                               uint32_t s0, uint32_t (&v)[8], Sink& sink) {
-  // (r2_run22, 45 MP frame with eight opcodes: the second walk 96.9 GPix/s, the first 88.6; both exact)
 #if defined(RSB200_DNGOP_V1)
   dngop_apply_group_v1(ops, nops, tables, deltas, jb, r, s0, v, sink);
 #elif defined(RSB200_DNGOP_V2)

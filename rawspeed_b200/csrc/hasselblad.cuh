@@ -1,4 +1,4 @@
-// hasselblad.cuh -- K2H: HasselbladDecompressor on the device (sm_100a).
+// hasselblad.cuh -- K2H: HasselbladDecompressor on the device (sm_90a).
 //
 // Reference: decompressors/HasselbladDecompressor.cpp:72-100 (decompress), :60-70 (getBits),
 // HasselbladLJpegDecoder.cpp:50-69; bit source BitStreamerMSB32 (bitstreams/BitStreamMSB32.h:

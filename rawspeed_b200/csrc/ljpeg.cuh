@@ -1,4 +1,4 @@
-// ljpeg.cuh -- K2 (JPEG entropy decode) + K3 (predictor-1 reconstruction), sm_100a.
+// ljpeg.cuh -- K2 (JPEG entropy decode) + K3 (predictor-1 reconstruction), sm_90a.
 //
 // Replaces the bodies of
 //   LJpegDecompressor::decodeN/decodeRowN   decompressors/LJpegDecompressor.cpp:184-339

@@ -1,5 +1,5 @@
 // ljpeg_clean.cuh -- K2C: unstuffing pre-pass of the one-thread-per-segment LJPEG
-// path (K2T, ljpeg_thread.cuh), sm_100a.
+// path (K2T, ljpeg_thread.cuh), sm_90a.
 //
 // One WARP per entropy-coded segment streams its raw bytes in pieces of 512 bytes
 // (one coalesced 128-bit load per lane, the next piece already in flight) and

@@ -1,5 +1,5 @@
 // ljpeg_fused.cuh -- K2F: fused LJPEG tile decode (entropy decode + predictor),
-// one CTA per entropy-coded segment, streaming in 8 KiB chunks (sm_100a).
+// one CTA per entropy-coded segment, streaming in 8 KiB chunks (sm_90a).
 //
 // Same semantics as k2_entropy_kernel + k3_* (see ljpeg.cuh for the reference
 // citations) but nothing but the compressed bytes is read from HBM and nothing

@@ -1,6 +1,6 @@
 // ljpeg_par.cuh -- K2P: LJPEG tile decode for SMALL launches (one frame ... a few dozen frames):
 // one CTA per entropy-coded segment, every thread parses a slice of the segment's CLEAN stream
-// (K2C, ljpeg_clean.cuh, has removed the stuffing), sm_100a.
+// (K2C, ljpeg_clean.cuh, has removed the stuffing), sm_90a.
 //
 // Same results as the other LJPEG kernels (reference: PrefixCodeLUTDecoder.h:172-216,
 // AbstractPrefixCodeDecoder.h:43-76, LJpegDecompressor.cpp:184-339).
@@ -314,8 +314,7 @@ par_body(ParShared& sh, const DevScan* __restrict__ scp, const DevTScan& ts, con
 
 // A CTA takes segments blockIdx.x, blockIdx.x + gridDim.x, ...: the plan launches one CTA per segment.
 // (A persistent grid of 2..5 CTAs per SM, so that the slices the resident CTAs walk fit the L1
-// cache, was measured SLOWER -- r2_run20: 0.50-0.66 ms per frame against 0.34 ms; the kernel wants
-// more warps in flight, not fewer: RSB200_PAR_CTAS keeps the experiment.)
+// cache, is the experiment RSB200_PAR_CTAS keeps: the kernel wants more warps in flight, not fewer.)
 __global__ void __launch_bounds__(P_NT)
     k2_par_kernel(const uint8_t* __restrict__ in, const DevScan* __restrict__ scans,
                   const DevTable* __restrict__ tables, uint8_t* __restrict__ out,

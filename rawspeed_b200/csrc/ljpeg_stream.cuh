@@ -1,5 +1,5 @@
 // ljpeg_stream.cuh -- K2S: LJPEG tile decode for LARGE batches, one THREAD per entropy-coded
-// segment, reading the RAW bytes (no unstuffing pre-pass), sm_100a.
+// segment, reading the RAW bytes (no unstuffing pre-pass), sm_90a.
 //
 // Same results as k2_thread_kernel / k2_fused_kernel (reference: PrefixCodeLUTDecoder.h:172-216,
 // AbstractPrefixCodeDecoder.h:43-76, LJpegDecompressor.cpp:184-339; the byte rules of the bit
@@ -412,14 +412,13 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 // therefore reduced to the windows that ALL of them resolve (stream_entry); a window dropped from
 // a LUT just takes the symbol-by-symbol path, which walks the code lengths.
 // RSB200_S_PIPE (A/B): the unit is bound by the ALU pipe (SHF / LOP3 / LEA / IADD3: one warp
-// instruction every two cycles; ncu at 256 frames: 76 % of its cycles against 25 % of the FMA pipe's,
-// profiles/r2_ncu_ljpeg.md).  ptxas turns every multiply by a constant power of two back into ALU
+// instruction every two cycles).  ptxas turns every multiply by a constant power of two back into ALU
 // forms, so the multipliers come from the constant bank (s_pipe_k), where it cannot see them:
 //   1: LUT address = (x >> 21) * 2 + base as SHF + IMAD (was LOP3 + LEA.HI); the sign mask from
 //      tt + 0x80000000 (IMAD) instead of ~tt (LOP3)
 //   2: + p + (e >> 10) and e >> 5 as IMAD.HI (were LEA.HI, SHF)
-// Measured (r2_run24, 256 frames, bit-exact): 0: 17.83 ms, 1: 17.18 ms (the default), 2: 18.26 ms
-// (IMAD.HI with a 64-bit addend costs two FMA-pipe instructions and is the slower form).
+// 1 is the default (IMAD.HI with a 64-bit addend costs two FMA-pipe instructions, which makes 2 the
+// slower form); not re-measured on H100.
 #ifndef RSB200_S_PIPE
 #define RSB200_S_PIPE 1
 #endif
@@ -490,23 +489,12 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 #ifndef RSB200_S_PREFETCH
 #define RSB200_S_PREFETCH 8 // blocks ahead of a requested sector that are pulled into L2 when the launch is small
 #endif
-#ifndef RSB200_S_LD256
-#define RSB200_S_LD256 1 // one 256-bit load per sector
-#endif
-#ifndef RSB200_S_ST256
-#define RSB200_S_ST256 1 // 0: never use the 256-bit stores (A/B)
-#endif
-
-__device__ __forceinline__ void stg_cs_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
-                                          uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
-#ifndef RSB200_EMU
-  asm volatile("st.global.cs.v8.u32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a), "r"(b), "r"(c),
-               "r"(d), "r"(e), "r"(f), "r"(g), "r"(h)
-               : "memory");
-#else
-  const uint32_t v[8] = {a, b, c, d, e, f, g, h};
-  memcpy(p, v, 32);
-#endif
+// One whole 32-byte sector of output: Hopper's widest store is 128 bits, so the two halves leave
+// back to back from the same lane.
+__device__ __forceinline__ void stg_cs_sector(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
+                                              uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
+  stg_cs_v4(p, make_uint4(a, b, c, d));
+  stg_cs_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
 }
 
 __device__ __forceinline__ void s_prefetch_l2(const void* p) {
@@ -517,22 +505,12 @@ __device__ __forceinline__ void s_prefetch_l2(const void* p) {
 #endif
 }
 
-// A lane's next two 16-byte blocks = one 32-byte sector, with ONE 256-bit load (sm_100:
-// LDG.E.ENL2.256).  Measured (ncu, 256 frames, profiles/r2_ncu_ljpeg.md): with a 16-byte load per
-// block 37 % of all warp samples sat on the first instruction that uses the block.  113 k streams
-// of lane-private requests are bound by the NUMBER of sector requests the memory system serves
-// (an L2 prefetch per block made small batches faster, -13 % at 32 frames, and full ones slower,
-// +6 % at 256 frames: it adds requests); asking for each sector once halves them.
+// A lane's next two 16-byte blocks = one 32-byte sector (blk even, cb 32-byte aligned): both
+// 128-bit loads are issued together, before the unit's decode that hides their latency.  113 k
+// streams of lane-private requests are bound by the number of requests the memory system serves,
+// so a lane asks for whole sectors and never for a block twice.
 __device__ __forceinline__ void s_ldg_sector(const uint4* cb, uint32_t blk, uint32_t bmax, uint4& a,
                                              uint4& b) {
-#if !defined(RSB200_EMU) && RSB200_S_LD256
-  if (blk < bmax) { // (blk even, cb 32-byte aligned; the last readable block may be the sector's first half)
-    asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(cb + blk));
-    return;
-  }
-#endif
   a = __ldg(cb + min(blk, bmax));
   b = __ldg(cb + min(blk + 1u, bmax));
 }
@@ -597,8 +575,8 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
   const uint32_t out_pitch = scp->out_pitch;
   uint8_t* orow = out + scp->out_offset + (uint64_t)scp->out_y * out_pitch + 2ull * scp->out_x;
   uint32_t bad = 0, last_tl = 0;
-  // (WIDE: pairs of units leave with one 256-bit store where the rows allow it)
-  const bool wide = WIDE && RSB200_S_ST256 && ((reinterpret_cast<uintptr_t>(orow) | out_pitch) & 31u) == 0u;
+  // (WIDE: pairs of units leave together as one 32-byte sector where the rows allow it)
+  const bool wide = WIDE && ((reinterpret_cast<uintptr_t>(orow) | out_pitch) & 31u) == 0u;
   uint32_t h0 = 0, h1 = 0, h2 = 0, h3 = 0;
 
   for (uint32_t r = 0; r < rows; ++r) {
@@ -697,15 +675,15 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
       }
       const uint32_t s = u << 3;
       // two units = one 32-byte sector of the output row: the even unit waits in registers for the
-      // odd one and both leave with one 256-bit store (half the write requests; r2_run13: 256 frames
-      // 20.7 -> 18.3 ms, but 32 frames 5.27 -> 5.64 ms: the plan picks by launch size)
+      // odd one and both leave back to back, so the sector is written whole at once (the plan
+      // picks WIDE by launch size)
       if (WIDE && wide && !(u & 1u) && s + 16u <= store_w) {
         h0 = o0;
         h1 = o1;
         h2 = o2;
         h3 = o3;
       } else if (WIDE && wide && (u & 1u) && s + 8u <= store_w) {
-        stg_cs_v8(orow + 16ull * (u - 1u), h0, h1, h2, h3, o0, o1, o2, o3);
+        stg_cs_sector(orow + 16ull * (u - 1u), h0, h1, h2, h3, o0, o1, o2, o3);
       } else if (s + 8 <= store_w) {
         stg_cs_v4(orow + 16ull * u, make_uint4(o0, o1, o2, o3));
       } else if (s < store_w) {

@@ -1,5 +1,5 @@
 // ljpeg_thread.cuh -- K2T: LJPEG tile decode for LARGE batches, one THREAD per
-// entropy-coded segment (DNG tile / restart interval), sm_100a.
+// entropy-coded segment (DNG tile / restart interval), sm_90a.
 //
 // Same results as k2_fused_kernel (see ljpeg.cuh / ljpeg_fused.cuh for the
 // reference citations: PrefixCodeLUTDecoder.h:172-216,

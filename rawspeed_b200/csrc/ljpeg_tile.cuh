@@ -1,5 +1,5 @@
 // ljpeg_tile.cuh -- K2G `k2_tile_kernel<R>`: lossless-JPEG tile decode (entropy decode +
-// predictor 1), one CTA per entropy-coded segment (DNG tile / restart interval), sm_100a.
+// predictor 1), one CTA per entropy-coded segment (DNG tile / restart interval), sm_90a.
 // Round-2 successor of k2_fused_kernel (ljpeg_fused.cuh) for the common shape of a DNG tile:
 // 1, 2 or 4 components in one MCU row, ONE Huffman table for all of them, rows that are whole
 // 8-sample units written with aligned 128-bit stores.  Everything else stays on k2_fused_kernel.
@@ -11,8 +11,8 @@
 //   AbstractPrefixCodeDecoder::processSymbol/extend  codes/AbstractPrefixCodeDecoder.h:43-76
 //   LJpegDecompressor::decodeN/decodeRowN   decompressors/LJpegDecompressor.cpp:184-339
 //
-// What changed against k2_fused_kernel, and why (profiles/r1_k2_fused.md: 5.1 warp-instructions
-// per pixel, every symbol decoded 2.9 times, 8-way bank conflicts on the clean buffer):
+// What changed against k2_fused_kernel, and why (it spends several warp-instructions per pixel,
+// decodes every symbol several times and meets 8-way bank conflicts on the clean buffer):
 //   * subsequences are LONG (~50 bytes for R = 1, ~100 for R = 2; an odd number of 32-bit words,
 //     so the 32 lanes of a warp read 32 different banks) and every thread except the first starts
 //     its length-only parse `preroll` bits BEFORE its subsequence: by the time it crosses into its
@@ -30,7 +30,7 @@
 //     end marker read as zero, and the segment only fails where BitStreamer::getInput would have
 //     thrown (position more than 16 bytes past the buffer at a refill), see tl_replay().
 //
-// The kernel body compiles for two targets: nvcc (sm_100a) and, with RSB200_EMU defined by
+// The kernel body compiles for two targets: nvcc (sm_90a) and, with RSB200_EMU defined by
 // tests/emu/cuda_emu.h, g++ -- the CPU replay the test-suite runs where there is no GPU.
 #pragma once
 
@@ -60,8 +60,8 @@ template <int R> struct TileGeom {
 #ifndef RSB200_TILE_DCAP1
 #define RSB200_TILE_DCAP1 15360
 #endif
-  // R = 1: 55 KB of shared memory -> four CTAs per SM (measured best: r2_run4; 168 / 11520 / 5 CTAs
-  // keeps all 726 tiles of a 45 MP frame resident at once but is slower); R = 2: 105 KB -> two
+  // R = 1: 55 KB of shared memory -> four CTAs per SM (an H100 SM has 228 KB, 227 KB of it for
+  // one block); R = 2: 105 KB -> two
   // CTAs per SM with subsequences twice as long
   static constexpr int NPIECE = R == 1 ? RSB200_TILE_NPIECE1 : 448; // pieces per chunk (at most)
   static constexpr int RAWMAX = NPIECE * TL_PIECE;   // raw bytes per chunk (at most)

@@ -1,10 +1,10 @@
-// pana.cuh -- K7: Panasonic RW2 block codecs V4 / V5 / V6 / V7 (SURVEY 8(f)4), sm_100a.
+// pana.cuh -- K7: Panasonic RW2 block codecs V4 / V5 / V6 / V7 (SURVEY 8(f)4), sm_90a.
 //
 // Replaces the bodies of
 //   PanasonicV4Decompressor::processBlock / processPixelPacket
 //       decompressors/PanasonicV4Decompressor.cpp:171-236 (+ ProxyStream :129-168); the
 //       packet arithmetic is in pana4_core.h.  (VER == 4 was developed against a CPU replay,
-//       tests/test_pana4_emu.py; first run on a B200: bit-exact, profiles/r1_postdecode_first_gpu_run.md.)
+//       tests/test_pana4_emu.py.)
 //   PanasonicV5Decompressor::processBlock / processPixelPacket
 //       decompressors/PanasonicV5Decompressor.cpp:188-232 (+ ProxyStream :147-186)
 //   PanasonicV6Decompressor::decompressBlock  PanasonicV6Decompressor.cpp:88-221

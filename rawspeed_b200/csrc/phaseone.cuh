@@ -1,4 +1,4 @@
-// phaseone.cuh -- K8: Phase One IIQ row codec (SURVEY 8(f)4), sm_100a.
+// phaseone.cuh -- K8: Phase One IIQ row codec (SURVEY 8(f)4), sm_90a.
 //
 // Replaces the body of PhaseOneDecompressor::decompressStrip
 // (decompressors/PhaseOneDecompressor.cpp:85-135) and the OpenMP loop over strips
@@ -298,8 +298,8 @@ __device__ __forceinline__ void p1_len_code_bf(uint32_t x, uint32_t& used, uint3
 
 // FAST: the window comes from three aligned words where they lie wholly inside the strip (all but the last
 // groups of a row), and the length codes are decoded without branches; !FAST: the first form of the walk
-// (generic chunk loads, branches), kept for A/B runs (RSB200_P1W=1).  r2_run25: the first form needs
-// about 170 instructions per group on a chain nobody hides.
+// (generic chunk loads, branches), kept for A/B runs (RSB200_P1W=1).  The first form needs about 170
+// instructions per group on a chain nobody hides.
 // A length code is decided by the 6 bits at the top of the window: 64 entries, bits used | a 1 bit came
 // before five zeros << 3 | new length << 4 (0: keep) -- one shared-memory load instead of a dozen
 // dependent instructions.
@@ -316,7 +316,7 @@ struct P1WalkShared {
 // TOUCH: every step also loads one word 192 bytes further down the row and uses it a step later (an XOR
 // into a value nobody needs): L1 is filled sector by sector on demand, and a row advances about half a
 // sector per group, so without it every second step waits for L2 and every fourth for DRAM, with nothing
-// else on the SM to run meanwhile (r2_run26: 1250 cycles per step).  The touch is ten steps ahead.
+// else on the SM to run meanwhile.  The touch is ten steps ahead.
 __device__ __forceinline__ void p1_prefetch(const void* q, int level) {
 #ifndef RSB200_EMU
   if (level == 1)
@@ -331,14 +331,14 @@ __device__ __forceinline__ void p1_prefetch(const void* q, int level) {
 
 // TOUCH: 0 nothing, 1 the look-ahead load described above, 2 prefetch.global.L1 192 bytes ahead, 3
 // prefetch.global.L2 512 bytes ahead + prefetch.global.L1 128 bytes ahead (no register waits for either),
-// 4 "blocks": ncu of form 3 (r2_run29): 13.4 cycles per instruction, 9.4 of them waiting for the three
-// lane-private window loads of every step although 92 % of their sectors hit L1.  So the row is read in
+// 4 "blocks": form 3 spends most of its cycles waiting for the three
+// lane-private window loads of every step although most of their sectors hit L1.  So the row is read in
 // aligned 16-byte blocks, two of them cached in registers (one 128-bit load every three to four steps, a
 // prefetch 192 bytes ahead at the same moment), the window's three words are selected from the eight
 // cached ones, and four descriptor words leave with one 128-bit store.  5 "lines": the row is read in
 // aligned lines of 128 bytes (eight 128-bit loads issued together, consumed a whole line -- about seven
 // steps -- later), two lines per row wait in shared memory and the window comes from there: the walk's
-// chain holds shared-memory loads only.  6 "cadence": ncu of "lines" (r2_run35): the rows of a warp cross
+// chain holds shared-memory loads only.  6 "cadence": in "lines" the rows of a warp cross
 // their line boundaries at different steps, so SOME lane refills at nearly every step, the whole warp runs
 // the refill code (twice the instructions) and -- the scoreboard of a load's destination register being
 // per warp -- every store of a pending line waits for the loads another lane issued a step ago.  So every
@@ -706,9 +706,8 @@ __global__ void __launch_bounds__(P1W_NT)
                    const P1JobDev* __restrict__ jobs, uint32_t gstride, uint32_t* __restrict__ gdesc,
                    uint32_t* __restrict__ rowflag, int first_form) {
   __shared__ P1WalkShared sh;
-  // 0 (default) = 7: "lines" (128-byte lines through a per-row ring in shared memory) -- the fastest of the
-  // forms measured (r2_run28 .. r2_run34, 101 MP frame: 1 first form 1.35 ms, 2 aligned words + table 1.20,
-  // 5 + look-ahead load 1.00, 3 + prefetch.global.L1 0.94, 4 two prefetches 0.94, 6 blocks 1.20, 7 lines 0.86)
+  // 0 (default) = 7: "lines" (128-byte lines through a per-row ring in shared memory), the form chosen
+  // during development; the forms have not been compared on H100
   if (first_form == 1)
     p1_walk_entry<false, 0>(sh, in, strips, nstrips, jobs, gstride, gdesc, rowflag);
   else if (first_form == 2)

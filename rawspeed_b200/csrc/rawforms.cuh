@@ -1,5 +1,5 @@
 // rawforms.cuh -- K1b: the fixed-layout forms of UncompressedDecompressor that are
-// not the generic N-bit bit pump (sm_100a).  Reference semantics, paths relative
+// not the generic N-bit bit pump (sm_90a).  Reference semantics, paths relative
 // to /root/reference/src/librawspeed:
 //   decode8BitRaw<uncorrected>            decompressors/UncompressedDecompressor.cpp:270-294
 //     (+ RawImageDataU16::setWithLookUp   common/RawImage.h:335-353)

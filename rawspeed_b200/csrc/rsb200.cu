@@ -1,4 +1,4 @@
-// rsb200.cu -- C ABI of the B200-native RAW decompression engine
+// rsb200.cu -- C ABI of the H100-native RAW decompression engine
 // (include/rawspeed_b200.h).  Host-side plan construction + kernel launches.
 // No CPU fallback lives here: every entry point needs a CUDA device.
 
@@ -317,7 +317,7 @@ struct rsb200_plan {
   int ntile = 0;
   int tile_r = 1;
   bool clean2 = false; // thread path: k2_clean2_kernel instead of k2_clean_kernel
-  int par_ctas = 0;        // k2_par_kernel: 0 = one CTA per segment; n = persistent, n CTAs per SM (RSB200_PAR_CTAS; measured slower, r2_run20)
+  int par_ctas = 0;        // k2_par_kernel: 0 = one CTA per segment; n = persistent, n CTAs per SM (RSB200_PAR_CTAS; an experiment)
   bool use_par = false;    // thread path for small launches: k2_clean_kernel + k2_par_kernel (one CTA per segment)
   bool use_stream = false; // thread path: k2_stream_kernel (unstuffing inside the thread) instead of K2C + K2T
   bool host_tiles_only = false; // tile_groups / d_tile_ids describe the thread path's segments for host-buffer runs only
@@ -365,8 +365,8 @@ extern "C" int rsb200_create(int device, rsb200_ctx** out) {
     e = cudaGetDeviceProperties(&prop, device);
     if (e == cudaSuccess) {
       c->sm_count = prop.multiProcessorCount;
-      if (prop.major < 10)
-        e = cudaErrorNoKernelImageForDevice; // sm_100a only, no fallback path
+      if (prop.major != 9 || prop.minor != 0)
+        e = cudaErrorNoKernelImageForDevice; // sm_90a only, no fallback path
     }
   }
   if (e == cudaSuccess)
@@ -1637,11 +1637,15 @@ constexpr uint32_t BIG_SEGMENT_BYTES = 256u << 10; // above this a segment gets 
 #ifndef RSB200_STREAM_DEFAULT
 #define RSB200_STREAM_DEFAULT 1
 #endif
-// k2_stream_kernel: an L2 prefetch ahead of every sector pays while the launch is latency bound
-// (r2_run12: 32 frames 6.67 -> 5.81 ms) and costs once the machine is full (128 frames 10.8 -> 11.9 ms)
+// k2_stream_kernel: an L2 prefetch ahead of every sector is meant for launches too small to fill the
+// machine (latency bound) and left out of full ones (it adds requests); the split, like the WIDE form of the
+// full launches (a pair of units leaves as two back-to-back 128-bit stores), has not been measured on H100
 constexpr size_t K2P_MAX_SEGMENTS = 0; // (k2_par_kernel: off by default until measured; RSB200_PAR_MAX / RSB200_LJPEG_PATH=par)
-constexpr int K2S_PREFETCH_MAX = 56832; // half a wave of 148 SMs x 6 CTAs x 128 threads
-constexpr size_t K2T_MIN_SEGMENTS = 16384; // measured crossover on B200: ~22 frames of 726 tiles
+// half a wave: for sm_90a ptxas gives k2_stream_kernel 80 registers, so 6 CTAs of 128 threads fit an SM
+constexpr int K2S_PREFETCH_CTAS_PER_SM = 3;
+// the thread path needs enough independent segments to fill the machine (~22 frames of 726 tiles); this
+// crossover has not been re-measured on H100
+constexpr size_t K2T_MIN_SEGMENTS = 16384;
 static bool thread_eligible(const DevScan& d) {
   return d.kind == 0 && d.pump == 0 && d.mcu_h == 1 &&
          (d.group == 1 || d.group == 2 || d.group == 4) && (d.row_samples & 7u) == 0 &&
@@ -1798,8 +1802,8 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
   p->nsmall = (int)small_ids.size();
   p->ntile = (int)tile_ids.size();
   // host-buffer runs of a plan made of tile-kernel segments only are pipelined: groups of
-  // consecutive segments worth ~16 MB of output each (32 MB in plans of more than 1 GB; measured,
-  // r2_run11: one frame 2.95 ms with 8 MB groups, 2.68 ms with 16 MB -- a download costs ~40 us + 23 us/MB)
+  // consecutive segments worth ~16 MB of output each (32 MB in plans of more than 1 GB): a download has a
+  // fixed cost of tens of microseconds, so groups must be large, and small enough to overlap
   auto build_groups = [&](const std::vector<uint32_t>& ids) {
     uint64_t total = 0;
     for (uint32_t i : ids)
@@ -1856,8 +1860,8 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
     uint64_t bytes = 0;
     for (uint32_t i : thread_ids)
       bytes += b.scans[i].in_size;
-    // measured (r2_run7, 256 frames): k2_clean_kernel 7.8 ms, k2_clean2_kernel ~12 ms (one CTA per
-    // segment is latency bound here) -> the warp-per-segment pre-pass stays the default
+    // the warp-per-segment pre-pass is the default: one CTA per small segment (k2_clean2_kernel) is
+    // latency bound
     (void)bytes;
     p->clean2 = false;
     if (const char* e = getenv("RSB200_CLEAN"))
@@ -2417,8 +2421,8 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
     }
     if (p->nthread && p->use_stream) {
       // small launches are latency bound (L2 prefetch ahead, 128-bit stores), full ones are bound
-      // by the number of memory requests (no prefetch, 256-bit stores)
-      if (p->nthread <= K2S_PREFETCH_MAX)
+      // by the number of memory requests (no prefetch, whole-sector stores)
+      if (p->nthread <= ctx->sm_count * K2S_PREFETCH_CTAS_PER_SM * T_NT)
         k2_stream_kernel<false><<<(p->nthread + T_NT - 1) / T_NT, T_NT, stream_smem_bytes(p->ntables), st>>>(
             in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
             p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 1);
@@ -3010,7 +3014,7 @@ static int gather_span(rsb200_comm* c, uint8_t* all, size_t slab, uint64_t lo, u
   if (!n || c->world == 1 || mode == RSB200_GATHER_NONE)
     return RSB200_OK;
   // Point-to-point transfers inside one group; a large span is cut into several of them so that
-  // NCCL spreads it over more channels (one ncclSend of 11.6 GB ran at 376 GB/s, r2_run6).
+  // NCCL spreads it over more channels.
   // GATHER_ALL = every rank sends its span to every other rank (all-gather with explicit
   // placement: slab r lands at the same offset everywhere).
   const size_t kPart = 32ull << 20;

@@ -1,4 +1,4 @@
-// scale.cuh -- K9: black/white level scaling of a decoded uint16 image, in place (sm_100a).
+// scale.cuh -- K9: black/white level scaling of a decoded uint16 image, in place (sm_90a).
 // Reference: RawImageDataU16::scaleValues (common/RawImageDataU16.cpp:185-399); the
 // per-lane arithmetic is in scale_core.h (shared with the CPU replay in tests/emu).
 //
@@ -8,8 +8,7 @@
 // sequential along a row, so every iteration starts with the 32 lanes advancing the 4 x 8
 // generators of the quad by 32 steps into the warp's private 1 KB of shared memory.
 //
-// Developed against a CPU replay of this loop (tests/test_scale_emu.py); first run on a B200:
-// bit-exact (profiles/r1_postdecode_first_gpu_run.md).
+// Developed against a CPU replay of this loop (tests/test_scale_emu.py).
 #pragma once
 
 #include "common.cuh"

@@ -1,4 +1,4 @@
-// sraw.cuh -- K5: Canon sRaw chroma interpolation + YCbCr -> RGB (sm_100a).
+// sraw.cuh -- K5: Canon sRaw chroma interpolation + YCbCr -> RGB (sm_90a).
 // Reference: interpolators/Cr2sRawInterpolator.cpp (paths relative to
 // /root/reference/src/librawspeed):
 //   YCbCr::process (sign-extend by 16384, add hue)            :66-86

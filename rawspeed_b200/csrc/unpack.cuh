@@ -1,4 +1,4 @@
-// unpack.cuh -- K1: packed N-bit -> uint16 (sm_100a).
+// unpack.cuh -- K1: packed N-bit -> uint16 (sm_90a).
 //
 // Replaces the body of UncompressedDecompressor::decodePackedInt<Pump>
 // (reference decompressors/UncompressedDecompressor.cpp:188-200) for the four

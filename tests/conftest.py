@@ -11,7 +11,7 @@ for p_ in (ROOT, HERE):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (B200); run on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (H100)")
 
 
 @pytest.fixture(scope="session")

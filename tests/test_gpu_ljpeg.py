@@ -205,16 +205,17 @@ def test_mixed_small_and_big_segments(ctx):
 
 
 def test_many_segments_take_the_thread_path(ctx, ljpeg_path):
-    """>= 16384 segments in one plan: the plan itself picks K2C + K2T (two launches)."""
-    if ljpeg_path != "auto":
-        pytest.skip("covered by the auto case")
+    """>= 16384 segments in one plan: the plan itself picks the one-thread-per-segment path; every
+    forced path decodes the same launch-sized batch bit for bit."""
     img = synth.image_model(4096, 4096, 51)
     t = synth.make_dng_ljpeg(img, 32, 32)
     tabs, scans = dng_ljpeg_scans(t, port.image_pitch(4096))
     assert len(scans) == 16384
     plan = rs.ljpeg_plan(ctx, tabs.tabs, scans)
-    # K2C + K2T, or k2_stream_kernel alone (32x32 tiles are below the tile kernel's row size: no second opinion)
-    assert plan.launches in (1, 2)
+    if ljpeg_path == "auto":
+        # K2C + K2T, or k2_stream_kernel alone (32x32 tiles are below the tile kernel's row size: no second opinion)
+        assert plan.launches in (1, 2)
+        assert "thread" in plan.kernels or "stream" in plan.kernels, plan.kernels
     got, res = gpu_run(plan, t.blob, port.new_image(4096, 4096))
     assert all(s == 0 for s, _ in res)
     want = port.new_image(4096, 4096)

@@ -1,7 +1,5 @@
 """The post-decode kernels (K9 scaling, K10 DNG opcodes, K11 bad pixels, K12 table lookup) and
-Panasonic V4 on the GPU, un-gated: exactly the two torch-free scripts that made their first
-contact with a B200 at the end of round 1 (profiles/r1_quick_validate_gpu.log,
-profiles/r1_quick_time_gpu.log), run as they ran there.
+Panasonic V4 on the GPU: the two torch-free scripts under tools/, run as a user would run them.
 
  * tools/quick_validate.py -- every scenario of their test files through the C++ host mirror
    (-> C ABI -> kernel), compared with the oracle: pixels, crops, bad-pixel lists in order,

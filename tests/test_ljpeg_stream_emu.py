@@ -29,7 +29,7 @@ DEPS = [SRC, os.path.join(HERE, "emu", "cuda_emu.h")] + [
 
 @pytest.fixture(scope="module", params=["default", "st256", "lut32", "pipe0", "pipe2"])
 def emu(request):
-    """The instantiations of the kernel: 128-bit output stores, 256-bit ones (two units per store), and
+    """The instantiations of the kernel: 128-bit output stores, whole 32-byte sectors (two units stored back to back), and
     the 32-bit LUT entries of the straight-line decode, and the FMA-pipe forms of its field arithmetic."""
     out = OUT if request.param == "default" else OUT.replace(".so", "_%s.so" % request.param)
     flags = {"default": [], "st256": ["-DRSB200_EMU_WIDE=true"],

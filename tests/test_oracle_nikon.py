@@ -7,7 +7,7 @@ import pytest
 import oracle
 from oracle import port, synth
 
-pytestmark = pytest.mark.skipif(not oracle.HAVE_REF, reason="reference build not available")
+pytestmark = pytest.mark.skipif(not oracle.REF_CHECKABLE, reason="reference build not available")
 
 
 def _case(kind, bits, w, h, be=True, seed=1):

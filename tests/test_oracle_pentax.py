@@ -8,7 +8,7 @@ import oracle
 from oracle import port, synth
 
 ref = oracle.ref
-pytestmark = pytest.mark.skipif(not oracle.HAVE_REF, reason="oracle/_ref/libref.so not built")
+pytestmark = pytest.mark.skipif(not oracle.REF_CHECKABLE, reason="oracle/_ref/libref.so not built")
 
 
 def both(img_shape, w, data, meta=None, meta_be=True):

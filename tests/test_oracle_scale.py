@@ -5,7 +5,7 @@ import pytest
 
 from oracle import port, ref
 
-needs_ref = pytest.mark.skipif(not ref.available(), reason="oracle/_ref/libref.so not built")
+needs_ref = pytest.mark.skipif(not ref.checkable(), reason="oracle/_ref/libref.so not built")
 
 
 def _image(w, h, seed, lo=0, hi=65536):

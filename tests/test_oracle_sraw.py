@@ -8,7 +8,7 @@ import oracle
 from oracle import port
 
 ref = oracle.ref
-pytestmark = pytest.mark.skipif(not oracle.HAVE_REF, reason="oracle/_ref/libref.so not built")
+pytestmark = pytest.mark.skipif(not oracle.REF_CHECKABLE, reason="oracle/_ref/libref.so not built")
 
 
 def sraw_input(num_mcus, rows, per, seed, extreme=False):
