@@ -37,17 +37,28 @@ __device__ __noinline__ uint2 t_slow_symbol(const DevTable* t, uint32_t x) {
                     (uint32_t)s.total | (s.codelen == 0 ? 0x80000000u : 0u));
 }
 
-// One difference at the top of window x with the LUT at shared address lutb
-// (slow path: table t).  Same arithmetic as f_decode_diff.
-__device__ __forceinline__ uint32_t t_decode_diff(const DevTable* t, uint32_t lutb, uint32_t x,
-                                                  uint32_t& tl, uint32_t& bad) {
+// The reference stops at the first unassigned code (RawDecoderException); the kernels decode on
+// behind it (one bit per such code) and keep the bit position where the first one began, bad_at
+// (T_NOBAD: none).  A code whose 16 bits lie wholly in the data is that verdict whatever follows.
+// One that reaches behind the end may be made of bits that are not the stream's (the reference
+// reads zeros there): then reading past the end decides, as for a segment without a bad code.
+constexpr uint32_t T_NOBAD = 0xFFFFFFFFu;
+__device__ __forceinline__ bool t_bad_in_data(uint32_t bad_at, uint32_t data_bits) {
+  return bad_at != T_NOBAD && bad_at + 16u <= data_bits;
+}
+
+// One difference at bit p, the top of window x, with the LUT at shared address lutb (slow path:
+// table t).  Same arithmetic as f_decode_diff.
+__device__ __forceinline__ uint32_t t_decode_diff(const DevTable* t, uint32_t lutb, uint32_t x, uint32_t p,
+                                                  uint32_t& tl, uint32_t& bad_at) {
   const uint32_t e =
       lds_u16<0>(mad_hi(x & ~((1u << (32 - LUT_BITS)) - 1u), 1u << (LUT_BITS + 1), lutb));
   tl = e >> 10;
   if (e == 0) { // code longer than the LUT, SSSS = 16, or corrupt
     const uint2 r = t_slow_symbol(t, x);
     tl = r.y & 0xFFu;
-    bad |= r.y >> 31;
+    if (r.y >> 31)
+      bad_at = min(bad_at, p);
     return r.x;
   }
   const uint32_t tt = __funnelshift_l(0u, x, e);

@@ -41,7 +41,7 @@ struct ParShared {
   uint32_t count[P_NT];
   uint32_t wtmp[P_NT / 32];
   uint32_t colbase[P_NT][4]; // per row chunk: exclusive column sums of the first MCU (4 components max)
-  uint32_t flags;            // bit 0: bad code among the needed symbols
+  uint32_t flags;            // bit 0: bad code wholly in the data among the needed symbols; bit 2: one that reaches behind it
 };
 
 // bits of the symbol at the top of window x (code + mantissa); 0x80000000 set: not a code
@@ -173,7 +173,7 @@ par_body(ParShared& sh, const DevScan* __restrict__ scp, const DevTScan& ts, con
         tl = e >> 10;
       } else {
         const SymLen s = decode_sym(tab, x);
-        bad |= s.codelen == 0 ? 1u : 0u;
+        bad |= s.codelen == 0 ? (p + 16u <= data_bits ? 1u : 4u) : 0u; // (see t_bad_in_data)
         d = (uint32_t)sym_diff(s, x) & 0xFFFFu;
         tl = (uint32_t)s.total;
       }
@@ -204,7 +204,7 @@ par_body(ParShared& sh, const DevScan* __restrict__ scp, const DevTScan& ts, con
       ++k;
     }
     if (bad)
-      atomicOr(&sh.flags, 1u);
+      atomicOr(&sh.flags, bad);
     if (k == n_samples && k > k0) { // I hold the last needed symbol
       sh.exitp[P_NT - 1] = tlast; // (slots of the chain are free now)
       sh.count[P_NT - 1] = plast;
@@ -215,13 +215,15 @@ par_body(ParShared& sh, const DevScan* __restrict__ scp, const DevTScan& ts, con
   const bool complete = (sh.flags & 2u) != 0u; // all needed symbols exist in the stream
   // status / consumed (as k2_thread_kernel)
   if (tid == 0) {
-    const bool bad = (sh.flags & 1u) != 0u;
+    const bool bad_in = (sh.flags & 1u) != 0u, bad = (sh.flags & 5u) != 0u;
     const uint32_t plast = complete ? sh.count[P_NT - 1] : 0xFFFFFFFFu;
     const bool over = !complete || plast > data_bits;
-    const bool again = over && !bad && redo && may_redo;
+    // (an unassigned code wholly in the data is the answer; one that reaches behind it is not, see
+    //  t_bad_in_data)
+    const bool again = over && !bad_in && redo && may_redo;
     if (redo)
       *redo = again ? 1u : 0u;
-    uint32_t status = bad ? 1u : ((over && !again) ? 2u : 0u);
+    uint32_t status = bad_in ? 1u : (over ? (again ? 0u : 2u) : (bad ? 1u : 0u));
     uint32_t consumed = 0;
     if (complete) {
       const uint64_t in_offset = scp->in_offset;
@@ -229,7 +231,7 @@ par_body(ParShared& sh, const DevScan* __restrict__ scp, const DevTScan& ts, con
       const uint32_t skew = (uint32_t)(in_offset - abase);
       consumed = t_stream_position(in + abase, skew + scp->in_size, skew, sh.exitp[P_NT - 1],
                                    anchors + ts.anchor_off, ts.n_anchor, info.clean_len);
-      if (!bad && !again && consumed > scp->in_size)
+      if (status != 1u && !again && consumed > scp->in_size)
         status = 2u; // the reference's skipBytes(consumed) behind the buffer
     }
     res->status = status;

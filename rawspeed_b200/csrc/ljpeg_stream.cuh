@@ -106,6 +106,28 @@ __device__ __forceinline__ void s_put_byte(SFill& f, uint32_t ringb, uint32_t b)
   }
 }
 
+// Once the data has ended, the ring bytes from data byte `clean_len` on become zero data, as the
+// reference reads them: the fast way puts a whole block into the ring, the bytes behind a marker too,
+// and the bytewise way has put the FF of a marker in as a data byte.
+// Otherwise a code that starts before the marker and reaches behind it could decode as unassigned
+// without its bits counting as missing.
+__device__ __noinline__ SFill s_zero_behind(SFill f, uint32_t ringb, uint32_t clean_len) {
+  const uint32_t stored = f.wo >> 7; // bytes in whole ring words
+  if (clean_len < stored) {
+#pragma unroll 1
+    for (uint32_t w = clean_len >> 2; w < (stored >> 2); ++w) {
+      const uint32_t keep = w == (clean_len >> 2) ? (clean_len & 3u) : 0u; // data bytes of the word
+      const uint32_t a = ringb + ((w * T_WSTRIDE) & T_RMASK);
+      sts_u32<0>(a, keep ? lds_u32<0>(a) & (~0u << (32u - 8u * keep)) : 0u);
+    }
+    f.acc = 0;
+  } else {
+    const uint32_t keep = clean_len - stored; // data bytes of the accumulator (left aligned)
+    f.acc = keep ? f.acc & (~0u << (32u - 8u * keep)) : 0u;
+  }
+  return f;
+}
+
 // One block the bytewise way: block 0 (the bytes before `skew` are not the segment's), the block
 // that holds raw offset `limit` (end of the buffer: what lies behind reads as zero data) and all
 // blocks once the data has ended.  The first marker ends the data (the FF before it was appended
@@ -148,6 +170,7 @@ __device__ __noinline__ SFill s_slow_block(SFill f, uint32_t ringb, uint32_t ein
   }
   f.pffm = carry ? 0x80000000u : 0u;
   if (f.clean_len != S_OPEN) {
+    f = s_zero_behind(f, ringb, f.clean_len); // (the FF of a marker went in as a data byte)
     f.slow_from = 0;
     f.pffm = 0;
     sts_u32<0>(einfo, blk);
@@ -278,6 +301,7 @@ __device__ __forceinline__ void s_block(SFill& f, uint32_t ringb, uint32_t selb,
     const uint32_t chk = s_fast_block(f, ringb, selb, q);
     if (chk != 0u) {
       const uint2 m = s_find_marker(gbase, blk, s_clean_count(f), skew);
+      f = s_zero_behind(f, ringb, m.x);
       f.clean_len = m.x;
       f.slow_from = 0;
       f.pffm = 0;
@@ -387,7 +411,7 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 #define S_SYM(c, val)                                                           \
   do {                                                                          \
     const uint32_t x_ = __funnelshift_l(nxt, cur, p);                           \
-    const uint32_t d_ = t_decode_diff(tabp[c], lutb[c], x_, last_tl, bad);      \
+    const uint32_t d_ = t_decode_diff(tabp[c], lutb[c], x_, p, last_tl, bad_at); \
     const uint32_t pn_ = p + last_tl;                                           \
     if ((pn_ ^ p) & 32u) { /* into the next word (a symbol is <= 32 bits) */    \
       cur = nxt;                                                                \
@@ -491,8 +515,14 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 #endif
 // One whole 32-byte sector of output: Hopper's widest store is 128 bits, so the two halves leave
 // back to back from the same lane.
+#ifdef RSB200_EMU
+inline unsigned long long g_emu_sector_stores = 0; // (CPU replay: how often the sector branch ran)
+#endif
 __device__ __forceinline__ void stg_cs_sector(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
                                               uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
+#ifdef RSB200_EMU
+  ++g_emu_sector_stores;
+#endif
   stg_cs_v4(p, make_uint4(a, b, c, d));
   stg_cs_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
 }
@@ -574,7 +604,7 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
   const uint32_t store_w = scp->store_w;
   const uint32_t out_pitch = scp->out_pitch;
   uint8_t* orow = out + scp->out_offset + (uint64_t)scp->out_y * out_pitch + 2ull * scp->out_x;
-  uint32_t bad = 0, last_tl = 0;
+  uint32_t bad_at = T_NOBAD, last_tl = 0;
   // (WIDE: pairs of units leave together as one 32-byte sector where the rows allow it)
   const bool wide = WIDE && ((reinterpret_cast<uintptr_t>(orow) | out_pitch) & 31u) == 0u;
   uint32_t h0 = 0, h1 = 0, h2 = 0, h3 = 0;
@@ -703,10 +733,13 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
   // by it (exact, tl_replay in ljpeg_tile.cuh); for the others the answer stays IOException
   // (DESIGN.md "known deviations").
   const bool over = p > 8u * f.clean_len;
-  const bool again = over && !bad && redo && may_redo;
+  // (an unassigned code wholly in the data is the answer; one that reaches behind it is not, see
+  //  t_bad_in_data)
+  const bool bad_in = t_bad_in_data(bad_at, 8u * f.clean_len);
+  const bool again = over && !bad_in && redo && may_redo;
   if (redo)
     *redo = again ? 1u : 0u;
-  res->status = bad ? 1u : ((over && !again) ? 2u : 0u);
+  res->status = bad_in ? 1u : (over ? (again ? 0u : 2u) : (bad_at != T_NOBAD ? 1u : 0u));
   {
     uint32_t ablk = f.nblk, acc = s_clean_count(f);
     if (f.clean_len != S_OPEN) {
@@ -718,7 +751,7 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
     // the reference skips `consumed` bytes of its input when the scan is done and throws when the
     // buffer is shorter (LJpegDecompressor.cpp:339 -> ByteStream::skipBytes): a buffer that ends
     // inside the last refill is an IOException even when every symbol was there
-    if (!bad && !again && consumed > scp->in_size)
+    if (res->status != 1u && !again && consumed > scp->in_size)
       res->status = 2u;
   }
 }

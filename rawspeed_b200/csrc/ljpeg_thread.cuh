@@ -86,7 +86,7 @@ __device__ __noinline__ uint32_t t_stream_position(const uint8_t* gbase, uint32_
 #define T_SYM(c, val)                                                           \
   do {                                                                          \
     const uint32_t x_ = __funnelshift_l(nxt, cur, p);                           \
-    const uint32_t d_ = t_decode_diff(tabp[c], lutb[c], x_, last_tl, bad);      \
+    const uint32_t d_ = t_decode_diff(tabp[c], lutb[c], x_, p, last_tl, bad_at); \
     const uint32_t pn_ = p + last_tl;                                           \
     if ((pn_ ^ p) & 32u) { /* into the next word (a symbol is <= 32 bits) */    \
       cur = nxt;                                                                \
@@ -136,7 +136,7 @@ thread_body(ThreadShared& sh, const DevScan* __restrict__ scp, const DevTScan& t
   const uint32_t store_w = scp->store_w;
   const uint32_t out_pitch = scp->out_pitch;
   uint8_t* orow = out + scp->out_offset + (uint64_t)scp->out_y * out_pitch + 2ull * scp->out_x;
-  uint32_t bad = 0, last_tl = 0;
+  uint32_t bad_at = T_NOBAD, last_tl = 0;
 
   for (uint32_t r = 0; r < rows; ++r) {
 #pragma unroll
@@ -220,10 +220,13 @@ thread_body(ThreadShared& sh, const DevScan* __restrict__ scp, const DevTScan& t
   // by it (exact, tl_replay in ljpeg_tile.cuh); for the others the answer stays IOException
   // (DESIGN.md "known deviations").
   const bool over = p > 8u * info.clean_len;
-  const bool again = over && !bad && redo && ts.pad;
+  // (an unassigned code wholly in the data is the answer; one that reaches behind it is not, see
+  //  t_bad_in_data)
+  const bool bad_in = t_bad_in_data(bad_at, 8u * info.clean_len);
+  const bool again = over && !bad_in && redo && ts.pad;
   if (redo)
     *redo = again ? 1u : 0u;
-  res->status = bad ? 1u : ((over && !again) ? 2u : 0u);
+  res->status = bad_in ? 1u : (over ? (again ? 0u : 2u) : (bad_at != T_NOBAD ? 1u : 0u));
   {
     const uint64_t in_offset = scp->in_offset;
     const uint64_t abase = in_offset & ~15ull;

@@ -320,6 +320,7 @@ struct rsb200_plan {
   int par_ctas = 0;        // k2_par_kernel: 0 = one CTA per segment; n = persistent, n CTAs per SM (RSB200_PAR_CTAS; an experiment)
   bool use_par = false;    // thread path for small launches: k2_clean_kernel + k2_par_kernel (one CTA per segment)
   bool use_stream = false; // thread path: k2_stream_kernel (unstuffing inside the thread) instead of K2C + K2T
+  int stream_form = 0;     // k2_stream_kernel: 0 = by launch size, 1 = prefetch form, 2 = full-launch form (RSB200_STREAM_FORM)
   bool host_tiles_only = false; // tile_groups / d_tile_ids describe the thread path's segments for host-buffer runs only
   std::vector<uint32_t> h_in_size; // per scan: bytes of a plain LJPEG segment (kind 0), else 0xFFFFFFFF
   DevTileParam* d_thread_tile_params = nullptr; // thread path: parameters of the exact second opinion
@@ -1643,6 +1644,14 @@ constexpr uint32_t BIG_SEGMENT_BYTES = 256u << 10; // above this a segment gets 
 constexpr size_t K2P_MAX_SEGMENTS = 0; // (k2_par_kernel: off by default until measured; RSB200_PAR_MAX / RSB200_LJPEG_PATH=par)
 // half a wave: for sm_90a ptxas gives k2_stream_kernel 80 registers, so 6 CTAs of 128 threads fit an SM
 constexpr int K2S_PREFETCH_CTAS_PER_SM = 3;
+// k2_stream_kernel<true> (no prefetch, whole-sector stores) for launches of more than half a wave of
+// thread-path segments, k2_stream_kernel<false> up to that; RSB200_STREAM_FORM overrides it
+static bool stream_full_launch(const rsb200_ctx* ctx, const rsb200_plan* p) {
+  if (p->stream_form)
+    return p->stream_form == 2;
+  const bool prefetch = p->nthread <= ctx->sm_count * K2S_PREFETCH_CTAS_PER_SM * T_NT;
+  return !prefetch;
+}
 // the thread path needs enough independent segments to fill the machine (~22 frames of 726 tiles); this
 // crossover has not been re-measured on H100
 constexpr size_t K2T_MIN_SEGMENTS = 16384;
@@ -1732,6 +1741,14 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
   }
   if (p->use_par)
     p->use_stream = false;
+  // RSB200_STREAM_FORM=prefetch|wide fixes the form of k2_stream_kernel whatever the launch size
+  // (stream_full_launch; tests run both forms on small batches)
+  if (const char* e = getenv("RSB200_STREAM_FORM")) {
+    if (!strcmp(e, "prefetch"))
+      p->stream_form = 1;
+    else if (!strcmp(e, "wide"))
+      p->stream_form = 2;
+  }
   // k2_tile_kernel<R> takes the plain single-table tiles; RSB200_LJPEG_PATH=fused keeps them on
   // k2_fused_kernel (tests run both), RSB200_TILE_R=1|2 picks the geometry, RSB200_TILE_PREROLL /
   // RSB200_TILE_NPIECES override the plan-time parameters (A/B runs)
@@ -2422,7 +2439,7 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
     if (p->nthread && p->use_stream) {
       // small launches are latency bound (L2 prefetch ahead, 128-bit stores), full ones are bound
       // by the number of memory requests (no prefetch, whole-sector stores)
-      if (p->nthread <= ctx->sm_count * K2S_PREFETCH_CTAS_PER_SM * T_NT)
+      if (!stream_full_launch(ctx, p))
         k2_stream_kernel<false><<<(p->nthread + T_NT - 1) / T_NT, T_NT, stream_smem_bytes(p->ntables), st>>>(
             in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
             p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 1);
@@ -3259,10 +3276,15 @@ extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
   if (only_thread && p->use_par)
     return "k2_clean_kernel + k2_par_kernel (one CTA per segment: speculative parse of the clean stream to a "
            "fixed point, decode, row sums)";
-  if (only_thread && p->use_stream)
-    return p->nthread_redo ? "k2_stream_kernel (one thread per segment, unstuffing in the thread) + "
+  if (only_thread && p->use_stream) {
+    if (stream_full_launch(p->ctx, p))
+      return p->nthread_redo ? "k2_stream_kernel (one thread per segment, unstuffing in the thread), full-launch form + "
+                               "k2_tile_kernel<1> for flagged ends of stream"
+                             : "k2_stream_kernel (one thread per segment, unstuffing in the thread), full-launch form";
+    return p->nthread_redo ? "k2_stream_kernel (one thread per segment, unstuffing in the thread), prefetch form + "
                              "k2_tile_kernel<1> for flagged ends of stream"
-                           : "k2_stream_kernel (one thread per segment, unstuffing in the thread)";
+                           : "k2_stream_kernel (one thread per segment, unstuffing in the thread), prefetch form";
+  }
   if (only_thread)
     return p->clean2 ? "k2_clean2_kernel + k2_thread_kernel (one thread per segment)"
                      : "k2_clean_kernel + k2_thread_kernel (one thread per segment)";

@@ -85,6 +85,12 @@ inline Cta*& cta() {
   return c;
 }
 
+// The global memory a kernel may read through __ldg: [ldg_lo, ldg_hi), set by a runner (unset: no
+// check).  A read outside it is counted and not performed (it returns zero).
+inline const uint8_t* ldg_lo = nullptr;
+inline const uint8_t* ldg_hi = nullptr;
+inline unsigned long long ldg_outside = 0;
+
 } // namespace cuemu
 
 // the CUDA built-ins the kernels read
@@ -290,7 +296,14 @@ static inline uint32_t __vcmpeq4(uint32_t a, uint32_t b) {
       r |= 0xFFu << (8 * i);
   return r;
 }
-template <typename T> static inline T __ldg(const T* p) { return *p; }
+template <typename T> static inline T __ldg(const T* p) {
+  const uint8_t* b = reinterpret_cast<const uint8_t*>(p);
+  if (cuemu::ldg_lo && (b < cuemu::ldg_lo || b + sizeof(T) > cuemu::ldg_hi)) {
+    ++cuemu::ldg_outside;
+    return T{};
+  }
+  return *p;
+}
 static inline long long clock64() { return 0; }
 static inline uint32_t atomicMin(uint32_t* p, uint32_t v) {
   const uint32_t o = *p;

@@ -9,26 +9,40 @@ from helpers import dng_ljpeg_scans, gpu_run
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(autouse=True, params=["auto", "tile2", "fused", "thread", "thread_clean2", "stream", "par"])
+LJPEG_PATHS = ["auto", "tile2", "fused", "thread", "thread_clean2", "stream", "stream_wide", "par"]
+
+
+@pytest.fixture(autouse=True, params=LJPEG_PATHS)
 def ljpeg_path(request, monkeypatch):
-    """Every case runs seven times: with the plan's own choice of kernel (k2_tile_kernel<1> for
+    """Every case runs eight times: with the plan's own choice of kernel (k2_tile_kernel<1> for
     plain single-table tiles, k2_fused_kernel for the rest, at these sizes), with the second
     geometry of the tile kernel (RSB200_TILE_R=2), with the round-1 block-per-segment kernel for
     everything (RSB200_LJPEG_PATH=fused), with the one-thread-per-segment path in its three
-    forms (K2C + K2T, K2C2 + K2T, and k2_stream_kernel which unstuffs inside the thread) and with
-    the one-CTA-per-segment speculative parse on the clean stream (K2C + k2_par_kernel)."""
+    forms (K2C + K2T, K2C2 + K2T, and k2_stream_kernel which unstuffs inside the thread), with
+    k2_stream_kernel in the form the plan gives full launches whatever the batch size (no L2
+    prefetch, whole-sector stores: RSB200_STREAM_FORM=wide) and with the one-CTA-per-segment
+    speculative parse on the clean stream (K2C + k2_par_kernel)."""
+    set_ljpeg_path(monkeypatch, request.param)
+    return request.param
+
+
+def set_ljpeg_path(monkeypatch, name):
+    """The environment of one of LJPEG_PATHS (tests/test_gpu_ljpeg_edges.py uses it as well)."""
     monkeypatch.delenv("RSB200_LJPEG_PATH", raising=False)
     monkeypatch.delenv("RSB200_TILE_R", raising=False)
     monkeypatch.delenv("RSB200_THREAD_KERNEL", raising=False)
+    monkeypatch.delenv("RSB200_STREAM_FORM", raising=False)
     monkeypatch.setenv("RSB200_CLEAN", "1")   # (the plan picks by segment size; here: both, explicitly)
-    if request.param == "tile2":
+    if name == "tile2":
         monkeypatch.setenv("RSB200_TILE_R", "2")
-    elif request.param == "thread_clean2":
+    elif name == "thread_clean2":
         monkeypatch.setenv("RSB200_LJPEG_PATH", "thread")
         monkeypatch.setenv("RSB200_CLEAN", "2")
-    elif request.param != "auto":
-        monkeypatch.setenv("RSB200_LJPEG_PATH", request.param)
-    return request.param
+    elif name == "stream_wide":
+        monkeypatch.setenv("RSB200_LJPEG_PATH", "stream")
+        monkeypatch.setenv("RSB200_STREAM_FORM", "wide")
+    elif name != "auto":
+        monkeypatch.setenv("RSB200_LJPEG_PATH", name)
 
 
 def _check_tiles(ctx, img, tile_w, tile_h, **kw):

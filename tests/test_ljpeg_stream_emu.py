@@ -8,6 +8,7 @@ test_ljpeg_tile_emu.py); every case that is NOT flagged must match the oracle in
 and pixels.
 Parity of the real kernel is the GPU tests' job (tests/test_gpu_ljpeg.py)."""
 import ctypes as C
+import itertools
 import os
 import subprocess
 
@@ -41,21 +42,39 @@ def emu(request):
         compile_shared(["g++", "-std=c++17", "-O2", "-Wall", "-Wno-unknown-pragmas",
                                "-Wno-unused-function", "-fPIC", "-shared"] + flags + ["-o", out, SRC])
     lib = C.CDLL(out)
-    lib.stream_emu_run.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
-                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.stream_emu_run.argtypes = [C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                   C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    lib.stream_emu_sector_stores.restype = C.c_ulonglong
+    lib.wide = request.param != "default"
     return lib
 
 
-def run_emu(lib, blob, tabs, scans, out, reverse=False, any_mode=0):
+def run_emu(lib, blob, tabs, scans, out, reverse=False, any_mode=0, in_base=0, out_base=0, may_redo=True):
+    """One launch of the replay.  in_base / out_base: the input and output buffers start at this
+    offset (0 or 16) from a 32-byte boundary; the replay copies them there itself.  may_redo=False: no
+    segment may be handed to the tile kernel (the plan's segments that it cannot take)."""
     tarr = (_abi.HuffTable * len(tabs))(*tabs)
     sarr = (_abi.LJpegScan * len(scans))(*scans)
     res = (_abi.ScanResult * len(scans))()
     redo = np.zeros(len(scans), dtype=np.uint32)
     blob = np.ascontiguousarray(blob)
-    rc = lib.stream_emu_run(blob.ctypes.data, blob.size, tarr, len(tabs), sarr, len(scans),
-                            out.ctypes.data, res, redo.ctypes.data, int(reverse), any_mode)
-    assert rc == 0, "emu rc %d (-1 = a scan is not eligible for the thread kernels)" % rc
+    assert out.flags.c_contiguous
+    rc = lib.stream_emu_run(blob.ctypes.data, blob.size, in_base, tarr, len(tabs), sarr, len(scans),
+                            out.ctypes.data, out.nbytes, out_base, res, redo.ctypes.data, int(reverse), any_mode,
+                            int(may_redo))
+    assert rc == 0, ("emu rc %d (-1 = a scan is not eligible for the thread kernels, "
+                     "-4 = a read outside the readable input)" % rc)
     return [(r.status, r.consumed, int(f)) for r, f in zip(res, redo)]
+
+
+def _sector_rows(scans, out_base):
+    """Whether the WIDE form stores whole 32-byte sectors for some segment: its first output row
+    and its pitch are 32-byte aligned, and a row holds at least two units."""
+    for s in scans:
+        row0 = out_base + s.out_offset + s.out_y * s.out_pitch + 2 * s.out_x
+        if ((row0 | s.out_pitch) & 31) == 0 and s.store_w >= 16 and s.rows > 0:
+            return True
+    return False
 
 
 def check_tiles(lib, img, tile_w, tile_h, **kw):
@@ -67,12 +86,21 @@ def check_tiles(lib, img, tile_w, tile_h, **kw):
     port.dng_decompress(t.blob, t.offsets, t.lengths, want, w, cpp, tile_w, tile_h, 7,
                         fix_ljpeg=kw.get("fix16", False), nthreads=4)
     tabs, scans = dng_ljpeg_scans(t, want.shape[1] * 2, fix16=kw.get("fix16", False))
-    for any_mode in (0, 1):
-        got = port.new_image(w, h, cpp)
-        res = run_emu(lib, t.blob, tabs.tabs, scans, got, reverse=bool(any_mode), any_mode=any_mode)
-        assert all(s == 0 and f == 0 for s, _, f in res), (any_mode, res[:4])
-        bad = np.argwhere(got != want)
-        assert bad.size == 0, (any_mode, bad[:5], got[tuple(bad[0])], want[tuple(bad[0])])
+    for out_base in (0, 16):
+        for any_mode in (0, 1):
+            got = port.new_image(w, h, cpp)
+            res = run_emu(lib, t.blob, tabs.tabs, scans, got, reverse=bool(any_mode), any_mode=any_mode,
+                          out_base=out_base)
+            assert all(s == 0 and f == 0 for s, _, f in res), (out_base, any_mode, res[:4])
+            bad = np.argwhere(got != want)
+            assert bad.size == 0, (out_base, any_mode, bad[:5], got[tuple(bad[0])], want[tuple(bad[0])])
+            # the WIDE form takes its sector branch exactly where rows and pitch are 32-byte aligned
+            # (output base 0 with a pitch that is a multiple of 32 bytes; never at base 16 for these tiles), the
+            # narrow form never
+            sectors = lib.stream_emu_sector_stores()
+            assert (sectors > 0) == (lib.wide and _sector_rows(scans, out_base)), (out_base, sectors)
+            if lib.wide and want.strides[0] % 32 == 0:
+                assert (sectors > 0) == (out_base == 0), (out_base, sectors)
     return t, tabs, scans
 
 
@@ -150,21 +178,22 @@ def test_stuffing_everywhere(emu):
 
 
 def test_many_offsets_of_the_segment_start(emu):
-    """The same tiles at every offset modulo 16 of the first byte (bytes before it in block 0)."""
+    """The same tiles at every offset modulo 32 of the first byte (bytes before it in the sector),
+    from an input base on a 32-byte boundary and from one 16 bytes behind it."""
     img = synth.image_model(256, 32, 31)
     t = synth.make_dng_ljpeg(img, 128, 32)
     tabs, scans = dng_ljpeg_scans(t, port.image_pitch(256))
     want = port.new_image(256, 32)
     port.dng_decompress(t.blob, t.offsets, t.lengths, want, 256, 1, 128, 32, 7, nthreads=1)
-    for shift in range(16):
+    for in_base, shift in itertools.product((0, 16), range(32)):
         blob = np.concatenate([np.full(shift, 0xFF, dtype=np.uint8), t.blob])
         sc = [rs.LJpegScan.from_buffer_copy(s) for s in scans]
         for s in sc:
             s.in_offset += shift
         got = port.new_image(256, 32)
-        res = run_emu(emu, blob, tabs.tabs, sc, got)
-        assert all(s == 0 and f == 0 for s, _, f in res), (shift, res)
-        assert np.array_equal(got, want), shift
+        res = run_emu(emu, blob, tabs.tabs, sc, got, in_base=in_base)
+        assert all(s == 0 and f == 0 for s, _, f in res), (in_base, shift, res)
+        assert np.array_equal(got, want), (in_base, shift)
 
 
 def test_consumed_matches_the_oracle(emu):
@@ -195,11 +224,11 @@ def _one_scan_outcome(s, data, hts, w, h):
         return 1, None, o
 
 
-def _check_against(emu, blob, tabs, s, want, w, h):
+def _check_against(emu, blob, tabs, s, want, w, h, in_base=0):
     want_status, want_cons, want_img = want
     for any_mode in (0, 1):
         got = port.new_image(w, h)
-        (status, consumed, redo), = run_emu(emu, blob, tabs.tabs, [s], got, any_mode=any_mode)
+        (status, consumed, redo), = run_emu(emu, blob, tabs.tabs, [s], got, any_mode=any_mode, in_base=in_base)
         if redo:
             assert status == 0   # handed to the tile kernel, which decides
             continue
@@ -244,20 +273,21 @@ def test_streams_with_an_early_marker(emu, cut):
 
 
 def test_marker_split_over_a_block_boundary(emu):
-    """FF as the last byte of a 16-byte block, D9 as the first of the next one -- at every offset."""
+    """FF as the last byte of a 16-byte block, D9 as the first of the next one -- at every offset
+    modulo 32, from both input bases."""
     img = synth.image_model(256, 32, 61)
     t = synth.make_dng_ljpeg(img, 256, 32)
     tabs, scans = dng_ljpeg_scans(t, port.image_pitch(256))
     hts = synth.default_tables(1)
     s0 = scans[0]
     end = s0.in_offset + s0.in_size
-    for shift in range(16):
+    for in_base, shift in itertools.product((0, 16), range(32)):
         blob = np.concatenate([np.zeros(shift, dtype=np.uint8), t.blob[:end]])
         s = rs.LJpegScan.from_buffer_copy(s0)
         s.in_offset += shift
         want = _one_scan_outcome(s, blob[s.in_offset:], hts, 256, 32)
         assert want[0] == 0
-        redo = _check_against(emu, blob, tabs, s, want, 256, 32)
+        redo = _check_against(emu, blob, tabs, s, want, 256, 32, in_base=in_base)
         assert redo == 0
 
 
@@ -283,6 +313,52 @@ def test_bad_huffman_code(emu):
     blob[s.in_offset + 40:s.in_offset + 49] = [0xFF, 0, 0xFF, 0, 0xFF, 0, 0xFF, 0, 0xFE]
     (status, _, redo), = run_emu(emu, blob, tabs.tabs, scans[:1], port.new_image(256, 32))
     assert (status, redo) == (1, 0)
+
+
+def inject_bad_code(data, rng, pos):
+    """An unassigned code of the default table at byte `pos` of entropy-coded data (in place): FF 00 FF 00 FE,
+    23 one-bits where no code of that table starts with more than 15, then 2 .. 11 random bytes that are not
+    FF, so that the decode behind the code goes on out of step.  The last two bytes (EOI) stay."""
+    junk = rng.integers(0, 255, int(rng.integers(2, 12)))
+    new = np.concatenate([[0xFF, 0, 0xFF, 0, 0xFE], junk]).astype(np.uint8)
+    if data[pos - 1] == 0xFF:    # (not between an FF and its stuffing byte)
+        pos += 1
+    n = max(0, min(new.size, data.size - 2 - pos))
+    data[pos:pos + n] = new[:n]
+
+
+@pytest.mark.parametrize("seed", range(4))
+def test_unassigned_code_then_a_run_past_the_end(emu, seed):
+    """A segment the tile kernel cannot take (may_redo cleared) with an unassigned code inside its data:
+    the kernel decodes on behind the code, out of step, and often runs past the end of the data.  The
+    reference throws at the code (RawDecoderException), so the kernel must report status 1, not the
+    IOException of a segment that merely ran out of data."""
+    img = synth.image_model(256, 32, 53)
+    t = synth.make_dng_ljpeg(img, 256, 32)
+    tabs, scans = dng_ljpeg_scans(t, port.image_pitch(256))
+    hts = synth.default_tables(1)
+    rng = np.random.default_rng(900 + seed)
+    n_rde = 0
+    for trial in range(25):
+        s = rs.LJpegScan.from_buffer_copy(scans[0])
+        data = t.blob[s.in_offset:s.in_offset + s.in_size].copy()
+        inject_bad_code(data, rng, int(rng.integers(8, data.size - 8)))
+        s.in_offset = 0
+        want_status, want_cons, want_img = _one_scan_outcome(s, data, hts, 256, 32)
+        for any_mode in (0, 1):
+            got = port.new_image(256, 32)
+            (status, consumed, redo), = run_emu(emu, data, tabs.tabs, [s], got, any_mode=any_mode, may_redo=False)
+            assert redo == 0
+            if want_status == 2:
+                assert status == 2, (trial, status)
+            elif want_status == 1:
+                assert status == 1, (trial, status)
+            else:   # (no second opinion: an end of stream the kernel cannot settle stays an IOException)
+                assert status in (0, 2), (trial, status)
+                if status == 0:
+                    assert consumed == want_cons and np.array_equal(got, want_img)
+        n_rde += want_status == 1
+    assert n_rde >= 20
 
 
 def _random_table(rng, nvalues, maxlen=16):
