@@ -178,6 +178,17 @@ struct BitSrc {
   }
 };
 
+// End of a plain MSB stream (DevScan::pump = 1: Pentax, Nikon).  BitStreamerMSB reads zero bits
+// behind the buffer and refills 4 bytes at a time; the refill that starts more than 8 bytes behind
+// the end throws (BitStreamer.h:100-131).  Those decoders refill to 32 bits before every code
+// (PrefixCodeDecoder), so before a code that starts at stream bit T the pump has done
+// (T >> 5) + 1 + (T & 31 ? 1 : 0) refills, and refill number (size + 8) / 4 + 2 is the one that
+// throws.  T only grows: the code of the segment's last sample decides.
+__device__ __forceinline__ bool plain_overread(uint64_t T, uint32_t size) {
+  const uint64_t refills = (T >> 5) + 1u + ((T & 31u) ? 1u : 0u);
+  return refills >= (uint64_t)((size + 8u) / 4u) + 2u;
+}
+
 // ------------------------------------------------------------------
 // K2: one CTA per segment
 // ------------------------------------------------------------------
@@ -309,6 +320,10 @@ __global__ void __launch_bounds__(K2_THREADS)
   const uint32_t skew = (uint32_t)(sc.in_offset - abase);
   const uint32_t* base = reinterpret_cast<const uint32_t*>(in + abase);
   const uint32_t limit = skew + sc.in_size;
+  // bytes behind the data in which a needed symbol may start: the JPEG pump keeps the rule of
+  // DESIGN.md "consumed"; for the plain pump plain_overread() decides, so the window only has to
+  // hold every symbol it allows (they start at most 8 bytes behind the data)
+  const uint32_t slack = sc.pump ? 16u : 8u;
   (void)in_total;
   if (tid == 0) {
     sh.carry_pos = skew * 8u;
@@ -327,13 +342,13 @@ __global__ void __launch_bounds__(K2_THREADS)
     const uint32_t carry_ff = sh.carry_ff;
     if (carry_sym >= sc.n_samples)
       break;
-    if (carry_pos == POS_END || (carry_pos >> 3) >= limit + 8u) {
+    if (carry_pos == POS_END || (carry_pos >> 3) >= limit + slack) {
       // ran out of data before all samples were decoded
       status |= 2u;
       break;
     }
     const uint32_t sub_byte = chunk * K2_CHUNK_BYTES + tid * SUBSEQ_BYTES;
-    const bool active = sub_byte < limit + 8u;
+    const bool active = sub_byte < limit + slack;
 
     // FF map of my subsequence (bit k = byte k is FF)
     uint32_t ffmask = 0;
@@ -442,7 +457,11 @@ __global__ void __launch_bounds__(K2_THREADS)
         if (s.total > bs.real_bits())
           status |= 2u; // symbol runs past the end marker
         dout[sym0 + k] = (uint16_t)sym_diff(s, x);
-        if (sym0 + k + 1 == sc.n_samples) {
+        if (sym0 + k + 1 == sc.n_samples && sc.pump != 0) {
+          // plain MSB pump: no stream position is reported, only its over-read rule
+          if (plain_overread(my_start - 8u * skew + consumed_bits, sc.in_size))
+            status |= 2u;
+        } else if (sym0 + k + 1 == sc.n_samples) {
           // ---- getStreamPosition() of the reference's pump after this, the
           // last, symbol (BitStreamer.h:216-229 refill cadence; see DESIGN.md)
           const uint32_t sb = my_start >> 3;

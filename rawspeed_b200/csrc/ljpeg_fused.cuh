@@ -649,7 +649,10 @@ __device__ __forceinline__ FSync f_sync(FusedShared& sh, uint32_t sb, const Fuse
                                         const FChunk& co, uint32_t G) {
   const int tid = threadIdx.x;
     const uint32_t sub_lo = tid * F_SUB * 8u;
-    const uint32_t sub_hi = min(sub_lo + F_SUB * 8u, co.end_all);
+    // the last thread also takes every symbol that starts behind the F_NT subsequences: a final
+    // chunk holds up to F_LA + F_RAW clean bytes (carried tail + chunk), and the range kernels parse
+    // a plain segment's final chunk a further 8 bytes into the zero bits
+    const uint32_t sub_hi = tid == F_NT - 1 ? co.end_all : min(sub_lo + F_SUB * 8u, co.end_all);
     const bool active = sub_lo < co.end_all;
     uint32_t my_start = (tid == 0) ? cy.pos : sub_lo;
     uint32_t my_phase = (tid == 0) ? (cy.sym % G) : 0u;
@@ -768,7 +771,7 @@ fused_body(FusedShared& sh, const uint8_t* __restrict__ in, uint64_t in_total,
     const uint32_t sincl = f_block_scan(d.count, sh.warp_tmp[3], &total_syms);
     const uint32_t sym0 = cy.sym + sincl - d.count; // global index of my first symbol
     const uint32_t chunk_syms = min(total_syms, sc.n_samples - cy.sym);
-    const uint32_t nsub = (end_all + F_SUB * 8u - 1) / (F_SUB * 8u);
+    const uint32_t nsub = min((end_all + F_SUB * 8u - 1) / (F_SUB * 8u), (uint32_t)F_NT);
     const uint32_t exit_all = nsub ? sh.exitpos[nsub - 1] : cy.pos;
     const uint32_t rel0 = sym0 - cy.sym;                     // chunk-relative index of my first symbol
     const uint32_t klast = sc.n_samples - 1 - cy.sym;        // chunk-relative index of the last needed one

@@ -17,8 +17,9 @@
 //              seam matches, induction from the exact start of range 0 proves
 //              the speculative parse IS the sequential parse; prefix sums then
 //              give every range its first symbol index.  If a seam does not
-//              match (possible in principle, never observed) a flag makes the
-//              exact single-CTA kernel (k2_entropy_kernel) redo that segment.
+//              match (not seen on camera data; tests/test_gpu_ljpeg_ranges.py
+//              forces it) a flag makes the exact single-CTA kernel
+//              (k2_entropy_kernel) redo that segment.
 //   P3 diffs   one CTA per range: decode from the verified entry state and write
 //              the differences in stream order; K3 (ljpeg.cuh) reconstructs and
 //              scatters through the CR2 slice map / tile crop.
@@ -132,6 +133,20 @@ __device__ __forceinline__ void r_stream(const FusedShared& sh, const uint8_t* i
   st.pending_par = 0;
 }
 
+// f_unstuff for the range kernels.  The plain MSB pump reads zero bits behind the data, and the
+// reference decodes codes that start there as long as the refill before them is allowed
+// (plain_overread): at the end of the segment, symbols that start up to 8 bytes behind the last
+// data byte are parsed too (ub holds 16 zero bytes behind the data).  The plain pump only comes
+// with one table (Pentax, Nikon): MULTI instantiations are plain f_unstuff.
+template <bool MULTI>
+__device__ __forceinline__ FChunk r_unstuff(FusedShared& sh, FStream& st, const FusedCarry& cy,
+                                            uint32_t chunk) {
+  FChunk co = f_unstuff(sh, st, cy, chunk);
+  if (!MULTI && st.plain && co.final_chunk && st.limit == st.skew + sh.sc.in_size)
+    co.end_all += 8u * 8u + 1u;
+  return co;
+}
+
 template <bool MULTI>
 __device__ __forceinline__ void range_count_body(FusedShared& sh, const uint8_t* in,
                                                  uint64_t in_total, uint32_t r,
@@ -167,11 +182,11 @@ __device__ __forceinline__ void range_count_body(FusedShared& sh, const uint8_t*
       break;
     mbar_wait(&sh.bar, (chunk - c_first) & 1u);
     st.pending = false;
-    const FChunk co = f_unstuff(sh, st, cy, chunk);
+    const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
     const FSync so = f_sync<MULTI>(sh, sb, cy, co, G);
     uint32_t total_syms;
     (void)f_block_scan(so.d.count, sh.warp_tmp[3], &total_syms);
-    const uint32_t nsub = (co.end_all + F_SUB * 8u - 1) / (F_SUB * 8u);
+    const uint32_t nsub = min((co.end_all + F_SUB * 8u - 1) / (F_SUB * 8u), (uint32_t)F_NT);
     const uint32_t exit_all = nsub ? sh.exitpos[nsub - 1] : cy.pos;
     // symbols that start inside the carried tail belong to the previous chunk
     uint32_t n_tail = 0, p_tail = cy.pos;
@@ -267,7 +282,7 @@ constexpr int V_NT = 256;
 __global__ void __launch_bounds__(V_NT)
     k2_range_verify_kernel(const DevScan* __restrict__ scans, const BigScanInfo* __restrict__ big,
                            const RangeState* __restrict__ states, RangeFinal* __restrict__ finals,
-                           uint32_t* __restrict__ fallback) {
+                           uint32_t* __restrict__ fallback, DevResult* __restrict__ results) {
   __shared__ uint32_t tmp[2][V_NT / 32];
   __shared__ uint32_t s_first_end, s_bad;
   const BigScanInfo bi = big[blockIdx.x];
@@ -344,8 +359,14 @@ __global__ void __launch_bounds__(V_NT)
     __syncthreads();
   }
   __syncthreads();
-  if (tid == 0)
+  if (tid == 0) {
     fallback[blockIdx.x] = s_bad;
+    // the data (and, for the plain pump, the zero bits the reference may read behind it) ends
+    // before the last sample: no range decodes it, so P3 cannot see it.  (With a failed seam the
+    // counts are speculative: k2_entropy_kernel redoes the segment and decides its status alone.)
+    if (base < N && !s_bad)
+      atomicOr(&results[bi.scan].status, 2u);
+  }
 }
 
 // ------------------------------------------------------------------ P3
@@ -389,14 +410,14 @@ __device__ __forceinline__ void range_diffs_body(FusedShared& sh, const uint8_t*
     }
     mbar_wait(&sh.bar, (chunk - c_own0) & 1u);
     st.pending = false;
-    const FChunk co = f_unstuff(sh, st, cy, chunk);
+    const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
     const FSync so = f_sync<MULTI>(sh, sb, cy, co, G);
     const FSub d = so.d;
     uint32_t total_syms;
     const uint32_t sincl = f_block_scan(d.count, sh.warp_tmp[3], &total_syms);
     const uint32_t sym0 = cy.sym + sincl - d.count;
     const uint32_t chunk_syms = min(total_syms, n_end - cy.sym);
-    const uint32_t nsub = (co.end_all + F_SUB * 8u - 1) / (F_SUB * 8u);
+    const uint32_t nsub = min((co.end_all + F_SUB * 8u - 1) / (F_SUB * 8u), (uint32_t)F_NT);
     const uint32_t exit_all = nsub ? sh.exitpos[nsub - 1] : cy.pos;
     const uint32_t rel0 = sym0 - cy.sym;
     const uint32_t klast = sc.n_samples - 1 - cy.sym; // the segment's very last symbol
@@ -426,9 +447,13 @@ __device__ __forceinline__ void range_diffs_body(FusedShared& sh, const uint8_t*
         plast = b.p;
         stop = dst_end;
       }
-      const uint32_t p = b.p;
-      if (co.final_chunk && p > co.len * 8u)
+      if (!MULTI && st.plain) {
+        // stream bit of the last code (plain: clean bytes are raw bytes)
+        if (plast != 0xFFFFFFFFu && plain_overread(8ull * cy.ubytes + plast, sc.in_size))
+          my_status |= 2u;
+      } else if (co.final_chunk && b.p > co.len * 8u) {
         my_status |= 2u;
+      }
       if (plast != 0xFFFFFFFFu && !st.plain) {
         // the reference's pump looks at the whole buffer, not just this range
         const uint32_t full_limit = st.skew + sc.in_size;

@@ -334,6 +334,7 @@ struct rsb200_plan {
   int nthread = 0;
   int ntables = 0;
   uint32_t* d_big_ids = nullptr;
+  std::vector<uint32_t> h_big_ids; // (for rsb200_debug_range_redo)
   int nbig = 0;
   BigScanInfo* d_big = nullptr;
   DevRange* d_ranges = nullptr;
@@ -1886,6 +1887,7 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
   }
   p->ntables = ntables;
   p->nbig = (int)big_ids.size();
+  p->h_big_ids = big_ids;
   p->nranges = (int)ranges.size();
   p->nrows = (uint32_t)b.rows.size();
   cudaError_t e = cudaSuccess;
@@ -2491,7 +2493,7 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
       k2_range_count_kernel<<<p->nranges, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans,
                                                            p->d_tables, p->d_ranges, p->d_states);
       k2_range_verify_kernel<<<p->nbig, V_NT, 0, st>>>(p->d_scans, p->d_big, p->d_states,
-                                                       p->d_finals, p->d_fallback);
+                                                       p->d_finals, p->d_fallback, p->d_results);
       k2_range_diffs_kernel<<<p->nranges, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans,
                                                            p->d_tables, p->d_ranges, p->d_finals,
                                                            p->d_diffs, p->d_results);
@@ -3221,6 +3223,30 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
   }
   return first;
+}
+
+// Debug entry (not in the public header; tests reach it through ctypes): after the last run of
+// `p`, flags[i] = 1 if scan i went through the multi-CTA range path (ljpeg_ranges.cuh) and a seam
+// failed its check, so that k2_entropy_kernel redid the whole segment; 0 otherwise (also for scans
+// that are not big).  Reads the flags P2 wrote; launches nothing.
+extern "C" int rsb200_debug_range_redo(const rsb200_plan* p, uint32_t* flags, int n) {
+  if (!p || n < 0 || (n > 0 && !flags))
+    return RSB200_ERR_ARG;
+  rsb200_ctx* ctx = p->ctx;
+  if (!p->ran)
+    return set_err(ctx, RSB200_ERR_ARG, "debug_range_redo: plan has not been run");
+  for (int i = 0; i < n; ++i)
+    flags[i] = 0;
+  if (p->h_big_ids.empty())
+    return RSB200_OK;
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
+  std::vector<uint32_t> fb(p->h_big_ids.size());
+  CUDA_TRY(ctx, cudaMemcpy(fb.data(), p->d_fallback, sizeof(uint32_t) * fb.size(), cudaMemcpyDeviceToHost));
+  for (size_t k = 0; k < fb.size(); ++k)
+    if ((int)p->h_big_ids[k] < n)
+      flags[p->h_big_ids[k]] = fb[k] ? 1u : 0u;
+  return RSB200_OK;
 }
 
 extern "C" int rsb200_plan_bad_pixels(rsb200_plan* p, int job, uint32_t* positions, uint32_t cap,
