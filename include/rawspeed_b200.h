@@ -504,6 +504,35 @@ int rsb200_pentax_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* tables, 
                               const rsb200_pentax_job* jobs, int njobs, rsb200_plan** plan);
 
 /* ------------------------------------------------------------------ */
+/* Sony ARW1 (SURVEY 8(f)2).                                             */
+/*   SonyArw1Decompressor::decompress  decompressors/SonyArw1Decompressor.cpp:58-92 */
+/*   (plain MSB bit stream, fixed prefix code, one running predictor    */
+/*   over the frame, walked column by column from the right: even rows, */
+/*   then odd rows; every value must stay in 0..4095).                  */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint64_t in_offset; /* first byte of the stream                                 */
+  uint32_t in_size;   /* bytes available (the rest of the file in ArwDecoder);   */
+                      /* < 2^28 (stream bit positions are 32-bit on the device)  */
+  uint32_t reserved0; /* 0                                                       */
+  int32_t width;      /* 1..4600 and height (even, 2..3072): the constructor's    */
+  int32_t height;     /* checks, SonyArw1Decompressor.cpp:39-50                   */
+  uint64_t out_offset; /* byte offset of image row 0 (even)                      */
+  uint32_t out_pitch;  /* bytes (even, >= 2 * width)                             */
+  uint32_t reserved;   /* 0                                                      */
+} rsb200_arw1_job;
+
+/* Dimensions the reference's constructor rejects fail plan creation with
+ * RSB200_ERR_RDE ("Unexpected image dimensions found").  rsb200_plan_results()
+ * for such a plan: RSB200_ERR_RDE with consumed == RSB200_PENTAX_OOB | (row << 14)
+ * | col = "Error decompressing" at the first pixel (stream order) whose value left
+ * 0..4095; RSB200_ERR_IOE = a refill of the bit pump started more than 8 bytes
+ * behind the stream, before that pixel, or a stream of fewer than 4 bytes.  Pixels up to the error are written, as
+ * the reference does; the rest of the image is left as it was. */
+int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* jobs, int njobs,
+                            rsb200_plan** plan);
+
+/* ------------------------------------------------------------------ */
 /* Nikon NEF Huffman codec without split (SURVEY 8(f)2).                 */
 /*   NikonDecompressor::decompress  decompressors/NikonDecompressor.cpp:513-560 */
 /*   (plain MSB bit stream, nikon_tree table, per-parity left predictor, */

@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -349,6 +349,14 @@ def pentax_plan(ctx, tables, jobs):
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_pentax_plan_create(ctx.h, ta, len(tables), ja, len(jobs),
                                                  C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def arw1_plan(ctx, jobs):
+    """Sony ARW1 streams (SonyArw1Decompressor::decompress), one job per frame."""
+    ja = (Arw1Job * len(jobs))(*jobs)
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_arw1_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

@@ -337,6 +337,21 @@ int rsb200h_pentax_decompress(uint16_t* img_data, int w, int h, int pitch, const
   });
 }
 
+int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
+                                 uint32_t size, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, 1, pitch, true, 1, 1);
+    SonyArw1Decompressor d(img);
+    try {
+      d.decompress(ByteStream(data, size));
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_nikon_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* meta,
                              uint32_t meta_size, int meta_be, int bitsPS, const uint8_t* data,
                              uint32_t size, int uncorrected, rsb200h_err* e) {

@@ -740,6 +740,44 @@ void PentaxDecompressor::decompress(ByteStream data) const {
   engineCheck(rc, "rsb200_plan_results");
 }
 
+// ------------------------------------------------------------------ Sony ARW1
+SonyArw1Decompressor::SonyArw1Decompressor(RawImage img) : mRaw(std::move(img)) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||
+      mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  const uint32_t w = mRaw->dim.x;
+  const uint32_t h = mRaw->dim.y;
+  if (w == 0 || h == 0 || h % 2 != 0 || w > 4600 || h > 3072)
+    ThrowRDE("Unexpected image dimensions found: (%u; %u)", w, h);
+}
+
+void SonyArw1Decompressor::decompress(ByteStream input) const {
+  if (input.getRemainSize() < 4) // BitStreamerMSB ctor (BitStreamer.h:56-60)
+    ThrowIOE("Bit stream size is smaller than MaxProcessBytes");
+  rsb200_arw1_job job;
+  std::memset(&job, 0, sizeof job);
+  job.in_offset = 0;
+  job.in_size = input.getRemainSize();
+  job.width = mRaw->dim.x;
+  job.height = mRaw->dim.y;
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  PlanGuard pg;
+  engineCheck(rsb200_arw1_plan_create(engine(), &job, 1, &pg.p), "rsb200_arw1_plan_create");
+  RawImage img = mRaw;
+  runOnImage(pg.p, input.begin() + input.getPosition(), input.getRemainSize(), img,
+             /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  if (res.status == RSB200_ERR_RDE)
+    ThrowRDE("Error decompressing"); // SonyArw1Decompressor.cpp:86-87
+  if (res.status == RSB200_ERR_IOE)
+    ThrowIOE("Buffer overflow read in BitStreamer");
+  engineCheck(rc, "rsb200_plan_results");
+}
+
 // ------------------------------------------------------------------ Nikon
 namespace {
 // NikonDecompressor::nikon_tree (NikonDecompressor.cpp:47-67)

@@ -581,6 +581,19 @@ private:
   const PrefixCodeDecoder<> ht;
 };
 
+// ---------------------------------------------------------------- Sony ARW1
+// decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
+// SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs
+// on the device (arw1.cuh); errors are thrown with the reference's classes.
+class SonyArw1Decompressor final {
+public:
+  explicit SonyArw1Decompressor(RawImage img);
+  void decompress(ByteStream input) const;
+
+private:
+  RawImage mRaw;
+};
+
 // ---------------------------------------------------------------- Nikon
 // decompressors/NikonDecompressor.h: same constructor (image, maker-note stream,
 // bits per sample) and decompress(input, uncorrectedRawValues).  The constructor work

@@ -644,9 +644,20 @@ struct FSync {
 };
 
 // ================= C: self-synchronising decode of the chunk in sh.ub =================
+// Sony ARW1 (arw1.cuh): a zero difference is the complemented code 100.  A parse that starts on
+// the wrong residue inside a run of them reads 001 (length 1) forever and never resynchronises, so
+// speculative starts inside such a run are moved to its phase (f_sync's arw1_align): the offset 0..2 at which the 32
+// bits of x0:x1 are 100 repeated, else 0.
+__device__ __forceinline__ uint32_t arw1_run_phase(uint32_t x0, uint32_t x1) {
+  for (uint32_t o = 0; o < 3; ++o)
+    if (__funnelshift_l(x1, x0, o) == 0x92492492u)
+      return o;
+  return 0;
+}
+
 template <bool MULTI>
 __device__ __forceinline__ FSync f_sync(FusedShared& sh, uint32_t sb, const FusedCarry& cy,
-                                        const FChunk& co, uint32_t G) {
+                                        const FChunk& co, uint32_t G, uint32_t arw1_align = 0) {
   const int tid = threadIdx.x;
     const uint32_t sub_lo = tid * F_SUB * 8u;
     // the last thread also takes every symbol that starts behind the F_NT subsequences: a final
@@ -656,6 +667,11 @@ __device__ __forceinline__ FSync f_sync(FusedShared& sh, uint32_t sb, const Fuse
     const bool active = sub_lo < co.end_all;
     uint32_t my_start = (tid == 0) ? cy.pos : sub_lo;
     uint32_t my_phase = (tid == 0) ? (cy.sym % G) : 0u;
+    // arw1_align: 1 = the guesses of threads 1.., 2 = thread 0's start too (a range's halo chunk);
+    // they stay guesses: the fixed point below is exact
+    if (arw1_align > (tid == 0 ? 1u : 0u) && active) // (thread 0: cy.pos == sub_lo == 0 then)
+      my_start += arw1_run_phase(sh.ub[sub_lo >> 5], sh.ub[(sub_lo >> 5) + 1]);
+    const uint32_t start0 = my_start; // thread 0's start (cy.pos unless aligned)
     if (!active)
       my_start = 0xFFFFFFF0u;
     FSub d;
@@ -672,7 +688,7 @@ __device__ __forceinline__ FSync f_sync(FusedShared& sh, uint32_t sb, const Fuse
     // With several tables the phase travels with the position hop by hop; once
     // positions are stable the phases come from a prefix sum of the counts.
     for (int round = 0; round < F_NT + 2; ++round) {
-      uint32_t new_start = (tid == 0) ? cy.pos : sh.exitpos[tid - 1];
+      uint32_t new_start = (tid == 0) ? start0 : sh.exitpos[tid - 1];
       uint32_t new_phase = my_phase;
       if (MULTI)
         new_phase = (tid == 0) ? (cy.sym % G) : sh.exitph[tid - 1];

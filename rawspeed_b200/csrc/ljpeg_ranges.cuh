@@ -183,7 +183,10 @@ __device__ __forceinline__ void range_count_body(FusedShared& sh, const uint8_t*
     mbar_wait(&sh.bar, (chunk - c_first) & 1u);
     st.pending = false;
     const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
-    const FSync so = f_sync<MULTI>(sh, sb, cy, co, G);
+    // ARW1: every speculative start follows a run of zero differences, including this CTA's guess at
+    // the start of its halo chunk
+    const uint32_t align = (!MULTI && sh.sc.kind == 4) ? ((chunk == c_first && r > 0) ? 2u : 1u) : 0u;
+    const FSync so = f_sync<MULTI>(sh, sb, cy, co, G, align);
     uint32_t total_syms;
     (void)f_block_scan(so.d.count, sh.warp_tmp[3], &total_syms);
     const uint32_t nsub = min((co.end_all + F_SUB * 8u - 1) / (F_SUB * 8u), (uint32_t)F_NT);
@@ -411,7 +414,7 @@ __device__ __forceinline__ void range_diffs_body(FusedShared& sh, const uint8_t*
     mbar_wait(&sh.bar, (chunk - c_own0) & 1u);
     st.pending = false;
     const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
-    const FSync so = f_sync<MULTI>(sh, sb, cy, co, G);
+    const FSync so = f_sync<MULTI>(sh, sb, cy, co, G, (!MULTI && sh.sc.kind == 4) ? 1u : 0u);
     const FSub d = so.d;
     uint32_t total_syms;
     const uint32_t sincl = f_block_scan(d.count, sh.warp_tmp[3], &total_syms);

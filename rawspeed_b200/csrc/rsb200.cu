@@ -28,6 +28,7 @@
 #include "phaseone.cuh"
 #include "pentax.cuh"
 #include "nikon.cuh"
+#include "arw1.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -347,6 +348,18 @@ struct rsb200_plan {
   uint32_t* h_oob = nullptr; // pinned
   bool has_pentax = false, has_k3 = false, has_nikon = false;
   uint16_t* d_nikon_luts = nullptr;
+  // Sony ARW1 frames (DevScan::kind == 4, arw1.cuh): the range decoder reads their complemented
+  // streams from d_arw1_in
+  bool has_arw1 = false;
+  int narw1 = 0;
+  DevArw1* d_arw1 = nullptr;
+  uint8_t* d_arw1_in = nullptr;
+  uint64_t arw1_in_bytes = 0;
+  Arw1Run* d_arw1_runs = nullptr;
+  uint32_t* d_arw1_lastoff = nullptr;
+  int2* d_arw1_runpre = nullptr;
+  Arw1Info* d_arw1_info = nullptr;
+  uint32_t arw1_max_runs = 0, arw1_max_tiles = 0, arw1_max_words = 0;
   cudaStream_t last_stream = nullptr;
   bool ran = false;
 };
@@ -1777,7 +1790,8 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
     DevScan& d = b.scans[i];
     const bool is_big = d.kind != 0 || d.in_size > BIG_SEGMENT_BYTES;
     if (is_big)
-      (d.kind == 2 ? p->has_pentax : (d.kind == 3 ? p->has_nikon : p->has_k3)) = true;
+      (d.kind == 2 ? p->has_pentax
+                   : (d.kind == 3 ? p->has_nikon : (d.kind == 4 ? p->has_arw1 : p->has_k3))) = true;
     if (!is_big) {
       if (use_thread && (p->use_par ? par_eligible(d) : thread_eligible(d))) {
         thread_ids.push_back((uint32_t)i);
@@ -1803,7 +1817,7 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
     d.col_offset = b.col_elems;
     b.col_elems += (uint64_t)d.rows * 4;
     d.row_begin = (uint32_t)b.rows.size();
-    for (uint32_t r = 0; r < d.rows; ++r)
+    for (uint32_t r = 0; d.kind != 4 && r < d.rows; ++r) // (ARW1: arw1.cuh reconstructs)
       b.rows.push_back(K3RowRef{(uint32_t)i, r});
     const uint32_t skew = (uint32_t)(d.in_offset & 15ull);
     const uint32_t range_bytes = (uint32_t)R_CHUNKS * F_RAW;
@@ -2037,6 +2051,128 @@ extern "C" int rsb200_pentax_plan_create(rsb200_ctx* ctx, const rsb200_huff_tabl
   int rc = finish_ljpeg_plan(ctx, p, tables, ntables, b, /*fused=*/false);
   if (rc != RSB200_OK)
     return rc;
+  *out = p;
+  return RSB200_OK;
+}
+
+// ------------------------------------------------------------------
+// Sony ARW1: one plain-MSB stream per frame (arw1.cuh: complemented copy, K2R, frame-wide scan)
+// ------------------------------------------------------------------
+// The prefix code of the complemented ARW1 stream (arw1.cuh): counts per code length 1..16 and
+// the extra bits of each code, in canonical order; length 17 is two 16-bit codes whose 16 extra
+// bits (DNG rule) make up its 17
+static rsb200_huff_table arw1_table() {
+  rsb200_huff_table t;
+  memset(&t, 0, sizeof t);
+  const uint8_t counts[16] = {0, 2, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2};
+  const uint8_t values[19] = {1, 2, 0, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 16, 16};
+  memcpy(t.ncodes_per_len, counts, sizeof counts);
+  memcpy(t.values, values, sizeof values);
+  t.nvalues = 19;
+  t.fix_dng16 = 1;
+  return t;
+}
+
+extern "C" int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* jobs, int njobs,
+                                       rsb200_plan** out) {
+  if (!ctx || !jobs || njobs <= 0 || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "arw1_plan_create: bad arguments");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_arw1_job& j = jobs[i];
+    // SonyArw1Decompressor ctor (SonyArw1Decompressor.cpp:39-50)
+    if (j.width <= 0 || j.height <= 0 || j.height % 2 != 0 || j.width > 4600 || j.height > 3072)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected image dimensions found: (%u; %u)", i,
+                     (unsigned)j.width, (unsigned)j.height);
+    if (j.in_size >= (1u << 28) || (uint64_t)j.width * 2 > j.out_pitch || (j.out_offset % 2) ||
+        (j.out_pitch % 2) || j.reserved0 || j.reserved)
+      return set_err(ctx, RSB200_ERR_ARG, "arw1 job %d: malformed descriptor", i);
+  }
+  rsb200_plan* p = new (std::nothrow) rsb200_plan();
+  if (!p)
+    return RSB200_ERR_CUDA;
+  p->ctx = ctx;
+  ScanBuild b;
+  std::vector<DevArw1> fr((size_t)njobs);
+  uint64_t koff = 0, runs = 0;
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_arw1_job& j = jobs[i];
+    const uint32_t w = (uint32_t)j.width, h = (uint32_t)j.height;
+    DevArw1& f = fr[(size_t)i];
+    memset(&f, 0, sizeof f);
+    f.in_offset = j.in_offset;
+    f.in_size = j.in_size;
+    f.k_offset = koff;
+    f.w = w;
+    f.h = h;
+    f.out_offset = j.out_offset;
+    f.out_pitch = j.out_pitch;
+    f.nrh = (h + 63) / 64;
+    // plain_overread (ljpeg.cuh): the first bit T with (T >> 5) + 1 + (T & 31 ? 1 : 0) refills
+    // >= (size + 8) / 4 + 2
+    f.tstar = 32u * ((j.in_size + 8u) / 4u) + 1u;
+    if (j.in_size < 4) // BitStreamerMSB's constructor throws (BitStreamer.h:56-60): before symbol 0
+      f.tstar = 0;
+    f.scan = (uint32_t)i;
+    f.run_offset = runs;
+    runs += (uint64_t)w * 2 * f.nrh;
+    p->arw1_max_runs = std::max(p->arw1_max_runs, w * 2 * f.nrh);
+    p->arw1_max_tiles = std::max(p->arw1_max_tiles, f.nrh * ((w + 63) / 64));
+    p->arw1_max_words = std::max(p->arw1_max_words, (j.in_size + 16u + 3u) / 4u);
+    DevScan d;
+    memset(&d, 0, sizeof d);
+    d.in_offset = koff;
+    d.in_size = j.in_size + 16u; // + the 0xFF bytes: zero bits of the original stream
+    d.row_samples = w;
+    d.rows = h;
+    d.n_samples = w * h;
+    d.group = 1;
+    d.ncomp = 1;
+    d.kind = 4;
+    d.pump = 1;
+    d.pattern = PAT_PLAIN;
+    const uint8_t tab[4] = {0, 0, 0, 0};
+    const uint8_t comp_of_pos[1] = {0};
+    assign_tables(d, tab, 1, comp_of_pos, 1);
+    d.out_offset = j.out_offset;
+    d.out_pitch = j.out_pitch;
+    d.mcu_w = 1;
+    d.mcu_h = 1;
+    d.store_w = w;
+    b.scans.push_back(d);
+    koff += ((uint64_t)j.in_size + 16u + 15u) & ~15ull;
+    p->in_bytes += j.in_size;
+    p->out_bytes += (uint64_t)w * h * 2;
+    p->pixels += (uint64_t)w * h;
+    p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
+    p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)h - 1) * j.out_pitch + 2ull * w));
+  }
+  const rsb200_huff_table t = arw1_table();
+  int rc = finish_ljpeg_plan(ctx, p, &t, 1, b, /*fused=*/false);
+  if (rc != RSB200_OK)
+    return rc;
+  for (size_t i = 0; i < fr.size(); ++i)
+    fr[i].diff_offset = b.scans[i].diff_offset;
+  p->narw1 = njobs;
+  p->arw1_in_bytes = koff;
+  cudaError_t e = rsb_dev_alloc((void**)&p->d_arw1, sizeof(DevArw1) * fr.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_arw1, fr.data(), sizeof(DevArw1) * fr.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_arw1_in, koff + 256);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_arw1_runs, sizeof(Arw1Run) * runs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_arw1_lastoff, sizeof(uint32_t) * runs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_arw1_runpre, sizeof(int2) * runs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_arw1_info, sizeof(Arw1Info) * fr.size());
+  if (e != cudaSuccess) {
+    rsb200_plan_destroy(p);
+    return set_err(ctx, RSB200_ERR_CUDA, "arw1 plan allocation failed: %s", cudaGetErrorString(e));
+  }
+  p->launches_per_run += 4;
   *out = p;
   return RSB200_OK;
 }
@@ -2490,16 +2626,25 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
     if (p->nbig) {
       k2_clear_results_kernel<<<(p->nbig + 127) / 128, 128, 0, st>>>(p->d_big, p->nbig,
                                                                      p->d_results, p->d_oob);
-      k2_range_count_kernel<<<p->nranges, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans,
+      // ARW1 frames: the range decoder reads the complemented copies (arw1.cuh)
+      const uint8_t* kin = in;
+      uint64_t kin_bytes = (uint64_t)in_bytes;
+      if (p->has_arw1) {
+        arw1_prep_kernel<<<dim3((p->arw1_max_words + 255) / 256, p->narw1), 256, 0, st>>>(
+            in, p->d_arw1_in, p->d_arw1);
+        kin = p->d_arw1_in;
+        kin_bytes = p->arw1_in_bytes;
+      }
+      k2_range_count_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans,
                                                            p->d_tables, p->d_ranges, p->d_states);
       k2_range_verify_kernel<<<p->nbig, V_NT, 0, st>>>(p->d_scans, p->d_big, p->d_states,
                                                        p->d_finals, p->d_fallback, p->d_results);
-      k2_range_diffs_kernel<<<p->nranges, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans,
+      k2_range_diffs_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans,
                                                            p->d_tables, p->d_ranges, p->d_finals,
                                                            p->d_diffs, p->d_results);
       // exact redo of segments whose speculative parse failed verification (no-op otherwise)
       k2_entropy_kernel<<<p->nbig, K2_THREADS, sizeof(K2Shared), st>>>(
-          in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->d_diffs, p->d_results,
+          kin, kin_bytes, p->d_scans, p->d_tables, p->d_diffs, p->d_results,
           p->d_big_ids, p->d_fallback);
       const int col_warps = p->nbig * 4;
       const uint32_t rows_per_block = K3_THREADS / 32;
@@ -2524,6 +2669,17 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
         k3n_row_kernel<<<(p->nrows + rows_per_block - 1) / rows_per_block, K3_THREADS, 0, st>>>(
             in, p->d_scans, p->d_rows, p->nrows, p->d_diffs, p->d_colvals, p->d_nikon_luts, outp);
         nk3 += 2;
+      }
+      if (p->has_arw1) {
+        arw1_runsum_kernel<<<dim3((p->arw1_max_runs + ARW1_NT / 32 - 1) / (ARW1_NT / 32), p->narw1),
+                             ARW1_NT, 0, st>>>(p->d_arw1, p->d_diffs, p->d_arw1_runs,
+                                               p->d_arw1_lastoff);
+        arw1_scan_kernel<<<p->narw1, ARW1_SCAN_NT, 0, st>>>(p->d_arw1, p->d_arw1_runs,
+                                                            p->d_arw1_lastoff, p->d_arw1_runpre,
+                                                            p->d_arw1_info, p->d_results);
+        arw1_apply_kernel<<<dim3(p->arw1_max_tiles, p->narw1), ARW1_NT, 0, st>>>(
+            p->d_arw1, p->d_diffs, p->d_arw1_runpre, p->d_arw1_info, outp, p->d_results);
+        nk3 += 4;
       }
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 5 + nk3;
@@ -3214,6 +3370,15 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
       results[i].status = p->h_results[i].status;
       results[i].consumed = p->h_results[i].consumed;
     }
+    if (first == RSB200_OK && p->h_results[i].status != 0 && p->has_arw1) {
+      // SonyArw1Decompressor.cpp:86-87 / BitStreamer.h:100-131
+      first = (int)p->h_results[i].status;
+      if (first == RSB200_ERR_RDE)
+        set_err(ctx, first, "job %d: Error decompressing (col %u, row %u)", i,
+                p->h_results[i].consumed & 0x3FFFu, (p->h_results[i].consumed >> 14) & 0xFFFu);
+      else
+        set_err(ctx, first, "job %d: Buffer overflow read in BitStreamer", i);
+    }
     if (first == RSB200_OK && p->h_results[i].status != 0) {
       first = (int)p->h_results[i].status;
       set_err(ctx, first,
@@ -3393,6 +3558,12 @@ extern "C" void rsb200_plan_destroy(rsb200_plan* p) {
   rsb_dev_free(p->d_finals);
   rsb_dev_free(p->d_fallback);
   rsb_dev_free(p->d_oob);
+  rsb_dev_free(p->d_arw1);
+  rsb_dev_free(p->d_arw1_in);
+  rsb_dev_free(p->d_arw1_runs);
+  rsb_dev_free(p->d_arw1_lastoff);
+  rsb_dev_free(p->d_arw1_runpre);
+  rsb_dev_free(p->d_arw1_info);
   if (p->h_oob)
     rsb_host_free(p->h_oob);
   if (p->h_results)
