@@ -89,8 +89,9 @@ typedef struct {
   uint64_t in_offset;  /* byte offset of the strip inside the input buffer       */
   uint64_t in_size;    /* bytes of the strip (>= rows*in_pitch; bytes past it read
                           as 0, BitStreamer.h:100-131)                           */
-  uint64_t out_offset; /* byte offset of image row 0 inside the output buffer    */
-  int32_t out_pitch;   /* bytes between output rows (RawImageData::pitch)        */
+  uint64_t out_offset; /* byte offset of image row 0 inside the output buffer;
+                          even                                                   */
+  int32_t out_pitch;   /* bytes between output rows (RawImageData::pitch); even  */
   int32_t row0;        /* first output row  (offset.y)                           */
   int32_t rows;        /* rows to decode    (min(h+oy, dim.y) - oy)              */
   int32_t samples;     /* samples per row   (size.x * cpp)                       */
@@ -134,8 +135,9 @@ enum {
 typedef struct {
   uint64_t in_offset;  /* byte offset of the strip inside the input buffer          */
   uint64_t in_size;    /* bytes of the strip (>= rows * in_pitch, checked)          */
-  uint64_t out_offset; /* byte offset of image row 0 inside the output buffer       */
-  int32_t out_pitch;   /* bytes between output rows                                 */
+  uint64_t out_offset; /* byte offset of image row 0 inside the output buffer; a
+                          multiple of the output sample size (2, or 4 for 7-11)     */
+  int32_t out_pitch;   /* bytes between output rows; a multiple of the sample size  */
   int32_t row0;        /* first output row                                          */
   int32_t rows;
   int32_t samples;     /* samples per row (w, or w*cpp for the float forms)         */
@@ -429,8 +431,8 @@ typedef struct {
   uint8_t table[4];   /* index into the plan's table array, per component       */
   uint8_t reserved[2];
   uint16_t init_pred[4]; /* PerComponentRecipe::initPred                        */
-  uint64_t out_offset;   /* byte offset of the image (row 0, col 0)             */
-  uint32_t out_pitch;    /* bytes                                               */
+  uint64_t out_offset;   /* byte offset of the image (row 0, col 0); even       */
+  uint32_t out_pitch;    /* bytes; even                                         */
   uint32_t out_x;        /* first output sample column = cpp * imgFrame.pos.x   */
   uint32_t out_y;        /* first output row of this segment                    */
   uint32_t store_w;      /* samples kept per row = cpp * imgFrame.dim.x         */
@@ -468,8 +470,8 @@ typedef struct {
   int32_t slice_w;           /*   columns, as passed to the Cr2Decompressor ctor   */
   int32_t last_slice_w;
   int32_t img_w, img_h;      /* RawImage dim (cpp == 1)                           */
-  uint64_t out_offset;
-  uint32_t out_pitch;
+  uint64_t out_offset;       /* byte offset of image row 0; even                  */
+  uint32_t out_pitch;        /* bytes; even, >= 2 * img_w                         */
   uint32_t reserved1;
 } rsb200_cr2_job;
 
@@ -621,7 +623,10 @@ int rsb200_hasselblad_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* tabl
 int rsb200_plan_launches(const rsb200_plan* plan);
 /* Which kernels one rsb200_plan_run() of this plan launches, as a short static string (for logs and
  * the benchmark's JSON line), e.g. "k2_stream_kernel (one thread per segment) [+ k2_tile_kernel<1>
- * second opinion]"; "" for a null plan. */
+ * second opinion]" for an LJPEG plan; "unpack_fast_kernel", "unpack_kernel" or
+ * "unpack_fast_kernel + unpack_kernel" for an unpack plan; "rawform_kernel" for a raw-form plan
+ * ("(empty unpack plan)" / "(empty raw-form plan)" when every job has 0 rows); "(not an LJPEG
+ * plan)" for the other kinds; "" for a null plan. */
 const char* rsb200_plan_kernels(const rsb200_plan* plan);
 void rsb200_plan_destroy(rsb200_plan* plan);
 

@@ -134,7 +134,7 @@ inline bool ljpeg_scan_to_dev(const rsb200_ljpeg_scan& s, int ntables, DevScan& 
   bool ok = mcu_ok && s.rows > 0 && s.frame_w > 0 && s.store_w > 0 &&
             (uint64_t)s.frame_w * s.mcu_w >= s.store_w &&
             ((uint64_t)s.out_x + (uint64_t)s.store_w) * 2 <= s.out_pitch &&
-            (s.out_offset & 1ull) == 0 &&
+            (s.out_offset & 1ull) == 0 && (s.out_pitch & 1u) == 0 &&
             (uint64_t)s.rows * s.frame_w * group < (1ull << 32) && s.in_size < (1u << 28) &&
             s.in_offset + (uint64_t)s.in_size >= s.in_offset;
   for (int c = 0; ok && c < group; ++c)

@@ -499,7 +499,7 @@ extern "C" int rsb200_unpack_plan_create(rsb200_ctx* ctx, const rsb200_unpack_jo
     const rsb200_unpack_job& j = jobs[i];
     if (j.bps < 1 || j.bps > 16 || j.order < 0 || j.order > 3 || j.rows < 0 ||
         j.samples <= 0 || j.in_pitch <= 0 || j.out_pitch <= 0 || j.row0 < 0 ||
-        j.out_col0 < 0 ||
+        j.out_col0 < 0 || (j.out_offset % 2) != 0 || (j.out_pitch % 2) != 0 ||
         ((uint64_t)j.samples * (uint64_t)j.bps) % 8 != 0 ||
         (uint64_t)j.in_pitch < ((uint64_t)j.samples * j.bps) / 8 ||
         (uint64_t)j.rows * (uint64_t)j.in_pitch > j.in_size ||
@@ -2366,7 +2366,8 @@ extern "C" int rsb200_cr2_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* 
               j.frame_h % j.y_s_f == 0 && j.num_slices >= 1 &&
               j.last_slice_w > 0 && (j.num_slices == 1 || j.slice_w > 0) &&
               j.slice_w % sliceColStep == 0 && j.last_slice_w % sliceColStep == 0 &&
-              (uint64_t)j.img_w * 2 <= j.out_pitch && j.in_size < (1u << 28);
+              (uint64_t)j.img_w * 2 <= j.out_pitch && (j.out_offset % 2) == 0 &&
+              (j.out_pitch % 2) == 0 && j.in_size < (1u << 28);
     for (int c = 0; ok && c < j.n_comp; ++c)
       ok = j.table[c] < ntables;
     DevScan d;
@@ -3460,6 +3461,17 @@ extern "C" int rsb200_plan_launches(const rsb200_plan* p) {
 extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
   if (!p)
     return "";
+  if (p->kind == 0) {
+    // jobs of bit depth 8/10/12/14/16 with 4-byte aligned input rows of >= 64 items (1024
+    // samples) take the fast kernel, the others the generic one
+    if (!p->fast_groups.empty() && !p->groups.empty())
+      return "unpack_fast_kernel + unpack_kernel";
+    if (!p->fast_groups.empty())
+      return "unpack_fast_kernel";
+    return p->groups.empty() ? "(empty unpack plan)" : "unpack_kernel";
+  }
+  if (p->kind == 2)
+    return p->raw_groups.empty() ? "(empty raw-form plan)" : "rawform_kernel";
   if (p->kind != 1)
     return "(not an LJPEG plan)";
   const bool only_thread = p->nthread && !p->ntile && !p->nsmall && !p->nbig;
