@@ -246,6 +246,47 @@ int rsb200_phaseone_plan_create(rsb200_ctx* ctx, const rsb200_phaseone_job* jobs
                                 rsb200_plan** plan);
 
 /* ------------------------------------------------------------------ */
+/* K13: Samsung SRW V0 row codec (SURVEY 8(f)4).                       */
+/*   SamsungV0Decompressor::decompress / decompressStrip                */
+/*   decompressors/SamsungV0Decompressor.cpp:92-204                     */
+/*   (one MSB32 bit stream per image row; blocks of 16 pixels predicted  */
+/*   from the left or from one / two rows above; red/blue swap after)   */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint64_t in_offset; /* first byte of the row's stream                           */
+  uint32_t in_size;   /* bytes of the row's stream (< 2^28)                       */
+  uint32_t reserved;  /* 0                                                        */
+} rsb200_samsung0_strip;
+
+typedef struct {
+  uint64_t out_offset;  /* byte offset of image row 0; even                       */
+  uint32_t out_pitch;   /* bytes between output rows; even, >= 2*width            */
+  uint32_t width;       /* 16..5546 and height 1..3714: the constructor's check   */
+  uint32_t height;      /* (SamsungV0Decompressor.cpp:51-55)                      */
+  uint32_t first_strip; /* its `height` strips, rows 0..height-1 in order, start
+                           here in the plan's strip array (computeStripes, :61-90) */
+} rsb200_samsung0_job;
+
+/* Dimensions the constructor rejects fail plan creation with RSB200_ERR_RDE
+ * ("Unexpected image dimensions found"); an odd out_offset or out_pitch, a pitch
+ * below 2*width or strips outside the array with RSB200_ERR_ARG.  Rows with 4-byte
+ * aligned out_offset and out_pitch are written 4 bytes at a time.
+ * rsb200_plan_results() per job: RSB200_ERR_RDE or RSB200_ERR_IOE with consumed ==
+ * code << 24 | row << 9 | block of the first failure (rows in order, blocks of 16
+ * pixels), code one of RSB200_S0_*.  The image is then as the reference leaves it:
+ * rows before the failing one decoded, that row up to the failing operation, the
+ * rest untouched, and no red/blue swap. */
+#define RSB200_S0_LEN_NEG 1u  /* RDE "Bit length less than 0."                             */
+#define RSB200_S0_LEN_BIG 2u  /* RDE "Bit Length more than 16."                            */
+#define RSB200_S0_UP_FIRST 3u /* RDE "Upward prediction for the first two rows. Raw corrupt" */
+#define RSB200_S0_UP_LAST 4u  /* RDE "Upward prediction for the last block of pixels. ..."   */
+#define RSB200_S0_OVERREAD 5u /* IOE "Buffer overflow read in BitStreamer"                  */
+#define RSB200_S0_SHORT 6u    /* IOE "Bit stream size is smaller than MaxProcessBytes"      */
+int rsb200_samsung0_plan_create(rsb200_ctx* ctx, const rsb200_samsung0_job* jobs, int njobs,
+                                const rsb200_samsung0_strip* strips, int nstrips,
+                                rsb200_plan** plan);
+
+/* ------------------------------------------------------------------ */
 /* K9: black / white level scaling, in place (SURVEY 8(f)3).            */
 /*   RawImageDataU16::scaleValues  common/RawImageDataU16.cpp:185-399   */
 /*   (the SCALE_VALUES worker of scaleBlackWhite(), :147-183)           */

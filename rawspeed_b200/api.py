@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -315,6 +315,16 @@ def phaseone_plan(ctx, jobs, strips):
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_phaseone_plan_create(ctx.h, ja, len(jobs), sa, len(strips),
                                                    C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def samsung0_plan(ctx, jobs, strips):
+    """Samsung SRW V0 row streams (SamsungV0Decompressor::decompress), one job per frame; job.first_strip
+    names the first of its `height` strips, rows in order."""
+    ja = (SamsungV0Job * len(jobs))(*jobs)
+    sa = (SamsungV0Strip * len(strips))(*strips)
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_samsung0_plan_create(ctx.h, ja, len(jobs), sa, len(strips), C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

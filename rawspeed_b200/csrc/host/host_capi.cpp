@@ -337,6 +337,21 @@ int rsb200h_pentax_decompress(uint16_t* img_data, int w, int h, int pitch, const
   });
 }
 
+int rsb200h_samsung_v0(uint16_t* img_data, int w, int h, int pitch, const uint8_t* bso, uint32_t bso_size,
+                       const uint8_t* bsr, uint32_t bsr_size, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, 1, pitch, true, 1, 1);
+    SamsungV0Decompressor d(img, ByteStream(bso, bso_size), ByteStream(bsr, bsr_size));
+    try {
+      d.decompress();
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
                                  uint32_t size, rsb200h_err* e) {
   return guarded(e, [&] {

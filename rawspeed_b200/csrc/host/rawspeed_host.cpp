@@ -740,6 +740,80 @@ void PentaxDecompressor::decompress(ByteStream data) const {
   engineCheck(rc, "rsb200_plan_results");
 }
 
+// ------------------------------------------------------------------ Samsung V0
+SamsungV0Decompressor::SamsungV0Decompressor(const RawImage& image, ByteStream bso, ByteStream bsr)
+    : mRaw(image) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||
+      mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  const uint32_t width = mRaw->dim.x;
+  const uint32_t height = mRaw->dim.y;
+  if (width == 0 || height == 0 || width < 16 || width > 5546 || height > 3714)
+    ThrowRDE("Unexpected image dimensions found: (%u; %u)", width, height);
+  computeStripes(bso.getStream(height, 4), bsr); // (peekStream of a copy: the same check)
+}
+
+// SamsungV0Decompressor::computeStripes (SamsungV0Decompressor.cpp:61-90)
+void SamsungV0Decompressor::computeStripes(ByteStream bso, ByteStream bsr) {
+  const uint32_t height = mRaw->dim.y;
+  std::vector<uint32_t> offsets;
+  offsets.reserve(1 + height);
+  for (uint32_t y = 0; y < height; y++)
+    offsets.emplace_back(bso.getU32());
+  offsets.emplace_back(bsr.getSize());
+  stripes.reserve(height);
+  bsr.skipBytes(offsets[0]);
+  for (uint32_t y = 0; y < height; y++) {
+    if (offsets[y] >= offsets[y + 1])
+      ThrowRDE("Line offsets are out of sequence or slice is empty.");
+    stripes.emplace_back(bsr.getStream(offsets[y + 1] - offsets[y]));
+  }
+}
+
+void SamsungV0Decompressor::decompress() const {
+  const uint32_t h = mRaw->dim.y;
+  const uint8_t* base = stripes[0].begin();
+  std::vector<rsb200_samsung0_strip> st(h);
+  for (uint32_t r = 0; r < h; ++r) {
+    st[r].in_offset = (uint64_t)(stripes[r].begin() - base);
+    st[r].in_size = stripes[r].getSize();
+    st[r].reserved = 0;
+  }
+  const size_t bytes = (size_t)(stripes[h - 1].begin() + stripes[h - 1].getSize() - base);
+  rsb200_samsung0_job job;
+  std::memset(&job, 0, sizeof job);
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  job.width = mRaw->dim.x;
+  job.height = h;
+  job.first_strip = 0;
+  PlanGuard pg;
+  engineCheck(rsb200_samsung0_plan_create(engine(), &job, 1, st.data(), (int)h, &pg.p),
+              "rsb200_samsung0_plan_create");
+  RawImage img = mRaw;
+  runOnImage(pg.p, base, bytes, img, /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  switch (res.consumed >> 24) { // SamsungV0Decompressor.cpp:147-160, BitStreamer.h:56-59, :96-104
+  case RSB200_S0_LEN_NEG:
+    ThrowRDE("Bit length less than 0.");
+  case RSB200_S0_LEN_BIG:
+    ThrowRDE("Bit Length more than 16.");
+  case RSB200_S0_UP_FIRST:
+    ThrowRDE("Upward prediction for the first two rows. Raw corrupt");
+  case RSB200_S0_UP_LAST:
+    ThrowRDE("Upward prediction for the last block of pixels. Raw corrupt");
+  case RSB200_S0_OVERREAD:
+    ThrowIOE("Buffer overflow read in BitStreamer");
+  case RSB200_S0_SHORT:
+    ThrowIOE("Bit stream size is smaller than MaxProcessBytes");
+  default:
+    engineCheck(rc, "rsb200_plan_results");
+  }
+}
+
 // ------------------------------------------------------------------ Sony ARW1
 SonyArw1Decompressor::SonyArw1Decompressor(RawImage img) : mRaw(std::move(img)) {
   if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||

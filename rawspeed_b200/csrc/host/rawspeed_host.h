@@ -581,6 +581,22 @@ private:
   const PrefixCodeDecoder<> ht;
 };
 
+// ---------------------------------------------------------------- Samsung V0
+// decompressors/SamsungV0Decompressor.h: same constructor (image, offset table bso, row data bsr;
+// its checks and computeStripes, SamsungV0Decompressor.cpp:44-90, on the host) and decompress().
+// The rows are decoded on the device (samsung0.cuh); errors are thrown with the reference's classes
+// and messages.
+class SamsungV0Decompressor final {
+public:
+  SamsungV0Decompressor(const RawImage& image, ByteStream bso, ByteStream bsr);
+  void decompress() const;
+
+private:
+  void computeStripes(ByteStream bso, ByteStream bsr);
+  RawImage mRaw;
+  std::vector<ByteStream> stripes;
+};
+
 // ---------------------------------------------------------------- Sony ARW1
 // decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
 // SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs

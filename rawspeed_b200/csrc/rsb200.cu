@@ -29,6 +29,7 @@
 #include "pentax.cuh"
 #include "nikon.cuh"
 #include "arw1.cuh"
+#include "samsung0.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -222,7 +223,7 @@ struct UnpackFastGroup {
 
 struct rsb200_plan {
   rsb200_ctx* ctx = nullptr;
-  int kind = 0; // 0 unpack, 1 ljpeg/cr2, 2 fixed-layout raw forms, 3 sRaw interpolation, 4 ARW2, 5 Panasonic, 6 Phase One, 7 black/white scaling (in place), 8 DNG opcode list (in place), 9 bad-pixel interpolation (in place), 10 whole-image table lookup (in place), 11 Hasselblad
+  int kind = 0; // 0 unpack, 1 ljpeg/cr2, 2 fixed-layout raw forms, 3 sRaw interpolation, 4 ARW2, 5 Panasonic, 6 Phase One, 7 black/white scaling (in place), 8 DNG opcode list (in place), 9 bad-pixel interpolation (in place), 10 whole-image table lookup (in place), 11 Hasselblad, 12 Samsung V0
   int nunits = 0;
   uint64_t in_bytes = 0, out_bytes = 0, pixels = 0;
   int launches_per_run = 0;
@@ -283,6 +284,19 @@ struct rsb200_plan {
   int p1_ver = 3;                   // which version of the kernel this plan runs (RSB200_P1)
   int p1_walk1 = 0;                 // RSB200_P1W = 1 .. 6: other forms of the third version's walk (A/B; see p1_walk_kernel)
   uint32_t p1_nstrips = 0;
+  // Samsung V0 (K13, samsung0.cuh)
+  S0RowDev* d_s0_rows = nullptr;
+  S0JobDev* d_s0_jobs = nullptr;
+  uint2* d_s0_desc = nullptr;     // per block
+  uint16_t* d_s0_adj = nullptr;   // per pixel (rows of 16 * blocks)
+  uint2* d_s0_nodes = nullptr;    // two ping-pong buffers of s0_nnodes
+  uint32_t* d_s0_carry = nullptr; // per row tile, column and chain
+  uint32_t* d_s0_rowfail = nullptr;
+  uint32_t* d_s0_jobfail = nullptr;
+  uint2* d_s0_res = nullptr;
+  uint2* h_s0_res = nullptr; // pinned
+  uint32_t s0_nrows = 0, s0_nnodes = 0, s0_max_nodes = 0, s0_max_w = 0, s0_max_tiles = 0;
+  int s0_rounds = 0;
   // Sony ARW2
   Arw2JobDev* d_arw2_jobs = nullptr;
   uint16_t* d_arw2_tables = nullptr;
@@ -1281,6 +1295,140 @@ static cudaError_t run_phaseone(const rsb200_plan* p, const uint8_t* in, uint8_t
         in, outp, p->d_p1_strips, p->p1_nstrips, p->d_p1_jobs, p->p1_gstride, p->d_p1_gdesc,
         p->d_p1_rowflag, p->d_arw2_bad);
   }
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------
+// Samsung V0 (K13): one MSB32 stream per row (samsung0.cuh)
+// ------------------------------------------------------------------
+extern "C" int rsb200_samsung0_plan_create(rsb200_ctx* ctx, const rsb200_samsung0_job* jobs, int njobs,
+                                           const rsb200_samsung0_strip* strips, int nstrips,
+                                           rsb200_plan** out) {
+  if (!ctx || !jobs || njobs <= 0 || !strips || nstrips <= 0 || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "samsung0_plan_create: bad arguments");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung0_job& j = jobs[i];
+    // SamsungV0Decompressor ctor (SamsungV0Decompressor.cpp:51-55)
+    if (j.width < 16 || j.width > 5546 || j.height == 0 || j.height > 3714)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected image dimensions found: (%u; %u)", i, j.width,
+                     j.height);
+    bool ok = (j.out_offset % 2) == 0 && (j.out_pitch % 2) == 0 && (uint64_t)j.width * 2 <= j.out_pitch &&
+              (uint64_t)j.first_strip + j.height <= (uint64_t)nstrips;
+    for (uint32_t r = 0; ok && r < j.height; ++r) {
+      const rsb200_samsung0_strip& st = strips[j.first_strip + r];
+      ok = st.in_size < (1u << 28) && st.reserved == 0;
+    }
+    if (!ok)
+      return set_err(ctx, RSB200_ERR_ARG, "samsung0 job %d: malformed descriptor or strips", i);
+  }
+  rsb200_plan* p = new (std::nothrow) rsb200_plan();
+  if (!p)
+    return RSB200_ERR_CUDA;
+  p->ctx = ctx;
+  p->kind = 12;
+  p->nunits = njobs;
+  std::vector<S0JobDev> dj((size_t)njobs);
+  std::vector<S0RowDev> dr;
+  uint64_t blk = 0, px = 0, carry = 0, nodes = 0;
+  uint32_t depth = 0;
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung0_job& j = jobs[i];
+    S0JobDev& d = dj[(size_t)i];
+    memset(&d, 0, sizeof d);
+    d.out_offset = j.out_offset;
+    d.out_pitch = j.out_pitch;
+    d.w = j.width;
+    d.h = j.height;
+    d.nb = (j.width + 15) / 16;
+    d.blk_base = blk;
+    d.px_base = px;
+    d.carry_base = carry;
+    d.node_base = (uint32_t)nodes;
+    d.row_base = (uint32_t)dr.size();
+    d.rtiles = (j.height + S0C_TH - 1) / S0C_TH;
+    blk += (uint64_t)d.h * d.nb;
+    px += (uint64_t)d.h * d.nb * 16;
+    carry += (uint64_t)d.rtiles * d.nb * 32;
+    nodes += (uint64_t)d.h * d.nb * 2;
+    depth = std::max(depth, d.h + d.nb + 1); // (a node chain moves up a row or left a block per step)
+    p->s0_max_nodes = std::max(p->s0_max_nodes, d.h * d.nb * 2);
+    p->s0_max_w = std::max(p->s0_max_w, d.w);
+    p->s0_max_tiles = std::max(p->s0_max_tiles, d.rtiles);
+    for (uint32_t r = 0; r < j.height; ++r) {
+      const rsb200_samsung0_strip& st = strips[j.first_strip + r];
+      dr.push_back(S0RowDev{st.in_offset, st.in_size, (uint32_t)i, r, 0});
+      p->in_bytes += st.in_size;
+      p->need_in = std::max<uint64_t>(p->need_in, sat_add(st.in_offset, st.in_size));
+    }
+    p->out_bytes += (uint64_t)j.width * j.height * 2;
+    p->pixels += (uint64_t)j.width * j.height;
+    p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch +
+                                                      2ull * j.width));
+  }
+  if (nodes >= S0_ROOT) {
+    delete p;
+    return set_err(ctx, RSB200_ERR_ARG, "samsung0 plan: too many frames for one plan");
+  }
+  p->s0_nrows = (uint32_t)dr.size();
+  p->s0_nnodes = (uint32_t)nodes;
+  while ((1u << p->s0_rounds) < depth)
+    ++p->s0_rounds;
+  cudaError_t e = rsb_dev_alloc(&p->d_s0_rows, sizeof(S0RowDev) * dr.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_s0_rows, dr.data(), sizeof(S0RowDev) * dr.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_jobs, sizeof(S0JobDev) * dj.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_s0_jobs, dj.data(), sizeof(S0JobDev) * dj.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_desc, sizeof(uint2) * blk);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_adj, sizeof(uint16_t) * px);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_nodes, sizeof(uint2) * 2 * nodes);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_carry, sizeof(uint32_t) * carry);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_rowfail, sizeof(uint32_t) * dr.size());
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_jobfail, sizeof(uint32_t) * (size_t)njobs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_res, sizeof(uint2) * (size_t)njobs);
+  if (e == cudaSuccess)
+    e = rsb_host_alloc((void**)&p->h_s0_res, sizeof(uint2) * (size_t)njobs);
+  if (e != cudaSuccess) {
+    rsb200_plan_destroy(p);
+    return set_err(ctx, RSB200_ERR_CUDA, "samsung0 plan allocation failed: %s", cudaGetErrorString(e));
+  }
+  p->launches_per_run = 6 + p->s0_rounds;
+  *out = p;
+  return RSB200_OK;
+}
+
+static cudaError_t run_samsung0(const rsb200_plan* p, const uint8_t* in, uint8_t* outp, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(p->d_s0_jobfail, 0xFF, sizeof(uint32_t) * (size_t)p->nunits, st);
+  if (e != cudaSuccess)
+    return e;
+  const uint32_t nj = (uint32_t)p->nunits;
+  s0_walk_kernel<<<(p->s0_nrows + S0W_NT - 1) / S0W_NT, S0W_NT, 0, st>>>(
+      in, p->d_s0_rows, p->s0_nrows, p->d_s0_jobs, p->d_s0_desc, p->d_s0_rowfail, p->d_s0_jobfail);
+  s0_diff_kernel<<<(p->s0_nrows + S0D_NT / 32 - 1) / (S0D_NT / 32), S0D_NT, 0, st>>>(
+      in, p->d_s0_rows, p->s0_nrows, p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj);
+  s0_node_kernel<<<dim3((p->s0_max_nodes + S0N_NT - 1) / S0N_NT, nj), S0N_NT, 0, st>>>(
+      p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, p->d_s0_nodes);
+  uint2* src = p->d_s0_nodes;
+  uint2* dst = p->d_s0_nodes + p->s0_nnodes;
+  for (int r = 0; r < p->s0_rounds; ++r) {
+    s0_jump_kernel<<<(p->s0_nnodes + S0N_NT - 1) / S0N_NT, S0N_NT, 0, st>>>(src, dst, p->s0_nnodes);
+    std::swap(src, dst);
+  }
+  const dim3 tiles((p->s0_max_w + S0C_NT - 1) / S0C_NT, p->s0_max_tiles, nj);
+  s0_scan_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, src, p->d_s0_carry);
+  s0_carry_kernel<<<dim3((2 * p->s0_max_w + S0C_NT - 1) / S0C_NT, nj), S0C_NT, 0, st>>>(p->d_s0_jobs,
+                                                                                     p->d_s0_carry);
+  s0_store_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, src, p->d_s0_carry,
+                                            p->d_s0_rowfail, p->d_s0_jobfail, outp, p->d_s0_res);
   return cudaGetLastError();
 }
 
@@ -2534,6 +2682,9 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
   } else if (p->kind == 6) {
     CUDA_TRY(ctx, run_phaseone(p, in, outp, st));
     ctx->launches++;
+  } else if (p->kind == 12) {
+    CUDA_TRY(ctx, run_samsung0(p, in, outp, st));
+    ctx->launches += (uint64_t)p->launches_per_run;
   } else if (p->kind == 5) {
     for (const PanaGroup& g : p->pana_groups) {
       CUDA_TRY(ctx, run_pana_group(p, g, in, outp, st));
@@ -3305,6 +3456,30 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
+  if (p->kind == 12) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_s0_res, p->d_s0_res, sizeof(uint2) * (size_t)p->nunits,
+                                  cudaMemcpyDeviceToHost, p->last_stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
+    static const char* const msgs[7] = {"", "Bit length less than 0.", "Bit Length more than 16.",
+                                        "Upward prediction for the first two rows. Raw corrupt",
+                                        "Upward prediction for the last block of pixels. Raw corrupt",
+                                        "Buffer overflow read in BitStreamer",
+                                        "Bit stream size is smaller than MaxProcessBytes"};
+    int first = RSB200_OK;
+    for (int i = 0; i < p->nunits; ++i) {
+      const uint2 r = p->h_s0_res[i];
+      if (results && i < n) {
+        results[i].status = r.x;
+        results[i].consumed = r.y;
+      }
+      if (r.x != RSB200_OK && first == RSB200_OK) {
+        first = (int)r.x;
+        set_err(ctx, first, "job %d: %s (row %u, block %u)", i, msgs[std::min(r.y >> 24, 6u)],
+                (r.y >> 9) & 0x7FFFu, r.y & 0x1FFu);
+      }
+    }
+    return first;
+  }
   if (p->kind == 11) {
     CUDA_TRY(ctx, cudaMemcpyAsync(p->h_hass_states, p->d_hass_states, sizeof(DevHassState) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
@@ -3472,6 +3647,9 @@ extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
   }
   if (p->kind == 2)
     return p->raw_groups.empty() ? "(empty raw-form plan)" : "rawform_kernel";
+  if (p->kind == 12)
+    return "s0_walk_kernel + s0_diff_kernel + s0_node_kernel + s0_jump_kernel + s0_scan_kernel + s0_carry_kernel + "
+           "s0_store_kernel";
   if (p->kind != 1)
     return "(not an LJPEG plan)";
   const bool only_thread = p->nthread && !p->ntile && !p->nsmall && !p->nbig;
@@ -3533,6 +3711,17 @@ extern "C" void rsb200_plan_destroy(rsb200_plan* p) {
   rsb_dev_free(p->d_hass_seg_job);
   rsb_dev_free(p->d_hass_u32);
   rsb_dev_free(p->d_hass_row_begin);
+  rsb_dev_free(p->d_s0_rows);
+  rsb_dev_free(p->d_s0_jobs);
+  rsb_dev_free(p->d_s0_desc);
+  rsb_dev_free(p->d_s0_adj);
+  rsb_dev_free(p->d_s0_nodes);
+  rsb_dev_free(p->d_s0_carry);
+  rsb_dev_free(p->d_s0_rowfail);
+  rsb_dev_free(p->d_s0_jobfail);
+  rsb_dev_free(p->d_s0_res);
+  if (p->h_s0_res)
+    rsb_host_free(p->h_s0_res);
   rsb_dev_free(p->d_p1_strips);
   rsb_dev_free(p->d_p1_jobs);
   rsb_dev_free(p->d_p1_gdesc);
