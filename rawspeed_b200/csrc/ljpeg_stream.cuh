@@ -513,18 +513,30 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 #ifndef RSB200_S_PREFETCH
 #define RSB200_S_PREFETCH 8 // blocks ahead of a requested sector that are pulled into L2 when the launch is small
 #endif
+// 128 bits of output with the default L2 policy.  A lane writes a 128-byte line of its output row
+// over eight (WIDE: four) store steps, microseconds apart; with evict-first stores (st.global.cs)
+// the kernel was about 2 % slower on H100 (DESIGN.md, K2S), presumably because L2 let such lines go
+// before they were whole.
+__device__ __forceinline__ void s_stg_v4(void* p, const uint4& v) {
+#ifdef RSB200_EMU
+  memcpy(p, &v, 16);
+#else
+  asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+               : "memory");
+#endif
+}
 // One whole 32-byte sector of output: Hopper's widest store is 128 bits, so the two halves leave
 // back to back from the same lane.
 #ifdef RSB200_EMU
 inline unsigned long long g_emu_sector_stores = 0; // (CPU replay: how often the sector branch ran)
 #endif
-__device__ __forceinline__ void stg_cs_sector(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
-                                              uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
+__device__ __forceinline__ void s_stg_sector(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
+                                             uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
 #ifdef RSB200_EMU
   ++g_emu_sector_stores;
 #endif
-  stg_cs_v4(p, make_uint4(a, b, c, d));
-  stg_cs_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
+  s_stg_v4(p, make_uint4(a, b, c, d));
+  s_stg_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
 }
 
 __device__ __forceinline__ void s_prefetch_l2(const void* p) {
@@ -535,14 +547,29 @@ __device__ __forceinline__ void s_prefetch_l2(const void* p) {
 #endif
 }
 
+// 128 bits of input through the read-only path, with an L2 fetch-size hint of 128 bytes: a miss
+// brings the rest of the 128-byte line into L2 with the sector asked for, and the lane reads it in
+// its next fill steps.  The hint adds no request (the explicit L2 prefetches of the small-launch form
+// make large launches more than twice as slow).
+__device__ __forceinline__ uint4 s_ldg_l2_128b(const uint4* p) {
+#ifdef RSB200_EMU
+  return __ldg(p);
+#else
+  uint4 r;
+  asm volatile("ld.global.nc.L2::128B.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+               : "l"(p));
+  return r;
+#endif
+}
 // A lane's next two 16-byte blocks = one 32-byte sector (blk even, cb 32-byte aligned): both
 // 128-bit loads are issued together, before the unit's decode that hides their latency.  113 k
 // streams of lane-private requests are bound by the number of requests the memory system serves,
 // so a lane asks for whole sectors and never for a block twice.
 __device__ __forceinline__ void s_ldg_sector(const uint4* cb, uint32_t blk, uint32_t bmax, uint4& a,
                                              uint4& b) {
-  a = __ldg(cb + min(blk, bmax));
-  b = __ldg(cb + min(blk + 1u, bmax));
+  a = s_ldg_l2_128b(cb + min(blk, bmax));
+  b = s_ldg_l2_128b(cb + min(blk + 1u, bmax));
 }
 
 template <int G, bool WIDE>
@@ -713,9 +740,9 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
         h2 = o2;
         h3 = o3;
       } else if (WIDE && wide && (u & 1u) && s + 8u <= store_w) {
-        stg_cs_sector(orow + 16ull * (u - 1u), h0, h1, h2, h3, o0, o1, o2, o3);
+        s_stg_sector(orow + 16ull * (u - 1u), h0, h1, h2, h3, o0, o1, o2, o3);
       } else if (s + 8 <= store_w) {
-        stg_cs_v4(orow + 16ull * u, make_uint4(o0, o1, o2, o3));
+        s_stg_v4(orow + 16ull * u, make_uint4(o0, o1, o2, o3));
       } else if (s < store_w) {
         uint16_t* o16 = reinterpret_cast<uint16_t*>(orow) + s;
         const uint32_t ow[4] = {o0, o1, o2, o3};
