@@ -47,17 +47,37 @@ constexpr uint32_t S_IDXMUL = (1u << 27) | (1u << 20) | (1u << 13) | (1u << 6);
 #define RSB200_S_LUT32 0 // 32-bit LUT entries laid out for IMAD.HI field extraction (A/B)
 #endif
 
+#ifndef RSB200_S_LB
+#define RSB200_S_LB 6 // CTAs per SM the kernel is compiled for (__launch_bounds__)
+#endif
+
 struct StreamShared {
   uint32_t sel[16];            // [remove flags of a word] -> PRMT selector | 8 * kept bytes << 16
   uint32_t endinfo[2][T_NT];   // per thread: block where the data ended, clean bytes before that block
   uint32_t ring[T_RING][T_NT]; // word w of a stream at ring[w % T_RING][thread]
   DevTable tab[T_MAXTAB];
   // (RSB200_S_LUT32: behind the tables in use, uint32_t lut32[ntab][1 << LUT_BITS])
+  // (where it fits, behind those: the output stage, S_STAGE bytes per thread, see s_flush)
 };
 
-__host__ __device__ inline size_t stream_smem_bytes(int ntab) {
+// Output staged per thread: 4 units = 32 samples = 64 bytes, which leave together as two whole sectors.
+constexpr uint32_t S_STAGE = 64;
+constexpr uint32_t H100_SMEM_PER_SM = 228u << 10;  // shared memory of an SM
+constexpr uint32_t H100_SMEM_PER_CTA_RESERVED = 1u << 10; // of it, reserved by the system per CTA
+
+// shared memory in front of the output stage: ring, tables (and the 32-bit LUTs)
+__host__ __device__ inline size_t stream_stage_offset(int ntab) {
   return sizeof(uint32_t) * (16 + 2 * T_NT + T_RING * T_NT) + sizeof(DevTable) * (size_t)ntab +
          (RSB200_S_LUT32 ? sizeof(uint32_t) * (size_t)ntab * (1u << LUT_BITS) : 0);
+}
+// The stage is there only when RSB200_S_LB CTAs with it still fit an SM (one or two tables); with more
+// tables a lane stores its units directly.
+__host__ __device__ inline bool stream_staged(int ntab) {
+  return (stream_stage_offset(ntab) + S_STAGE * T_NT + H100_SMEM_PER_CTA_RESERVED) * RSB200_S_LB <=
+         H100_SMEM_PER_SM;
+}
+__host__ __device__ inline size_t stream_smem_bytes(int ntab) {
+  return stream_stage_offset(ntab) + (stream_staged(ntab) ? S_STAGE * T_NT : 0);
 }
 // LUT entry for the straight-line decode: [4:0] code length, [12:8] SSSS, bit 16 = 1 (a hit; eight
 // of them add up in a counter without touching the other fields' sums), [31:26] bits of code +
@@ -514,8 +534,8 @@ __device__ __forceinline__ bool s_any(bool want) { return __any_sync(__activemas
 #define RSB200_S_PREFETCH 8 // blocks ahead of a requested sector that are pulled into L2 when the launch is small
 #endif
 // 128 bits of output with the default L2 policy.  A lane writes a 128-byte line of its output row
-// over eight (WIDE: four) store steps, microseconds apart; with evict-first stores (st.global.cs)
-// the kernel was about 2 % slower on H100 (DESIGN.md, K2S), presumably because L2 let such lines go
+// over two to eight store steps, microseconds apart; with evict-first stores (st.global.cs) the
+// kernel was about 2 % slower on H100 (DESIGN.md, K2S), presumably because L2 let such lines go
 // before they were whole.
 __device__ __forceinline__ void s_stg_v4(void* p, const uint4& v) {
 #ifdef RSB200_EMU
@@ -525,10 +545,20 @@ __device__ __forceinline__ void s_stg_v4(void* p, const uint4& v) {
                : "memory");
 #endif
 }
+
+// Unit j (0..3) of a group sits at 16 * (j ^ ((lane >> 1) & 3)) in the lane's 64-byte stage: the
+// 128-bit shared accesses of a quarter warp (8 lanes) then hit 8 different 16-byte bank groups, both
+// when each lane writes one unit of its own stage and when four lanes read one stage (s_flush).
+__device__ __forceinline__ uint32_t s_stage_unit(uint32_t lane, uint32_t j) {
+  return 16u * ((j ^ (lane >> 1)) & 3u);
+}
+
 // One whole 32-byte sector of output: Hopper's widest store is 128 bits, so the two halves leave
 // back to back from the same lane.
 #ifdef RSB200_EMU
-inline unsigned long long g_emu_sector_stores = 0; // (CPU replay: how often the sector branch ran)
+// (CPU replay: whole 32-byte sectors of segments whose rows are 32-byte aligned, stored by this branch
+//  or as a staged run)
+inline unsigned long long g_emu_sector_stores = 0;
 #endif
 __device__ __forceinline__ void s_stg_sector(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d,
                                              uint32_t e, uint32_t f, uint32_t g, uint32_t h) {
@@ -537,6 +567,52 @@ __device__ __forceinline__ void s_stg_sector(void* p, uint32_t a, uint32_t b, ui
 #endif
   s_stg_v4(p, make_uint4(a, b, c, d));
   s_stg_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
+}
+
+// "every lane of my warp is here" -- a hint only: results do not depend on it (s_flush)
+#ifdef RSB200_EMU
+inline unsigned long long g_emu_runs_shared = 0; // (CPU replay: 64-byte runs stored by the whole warp)
+inline unsigned long long g_emu_runs_own = 0;    // (... by the lane whose run it is)
+// a replay that gathers the lanes of a warp defines this; otherwise every lane is alone
+#ifndef RSB200_EMU_WHOLE_WARP
+#define RSB200_EMU_WHOLE_WARP() false
+#endif
+__device__ __forceinline__ bool s_whole_warp() { return RSB200_EMU_WHOLE_WARP(); }
+#else
+__device__ __forceinline__ bool s_whole_warp() { return __activemask() == 0xFFFFFFFFu; }
+#endif
+// The lane's last four units (its stage) go to `dst` (16-byte aligned).  Where the whole warp is here,
+// the lanes store each other's stages: lane l writes 16 bytes of the run of lane 8k + l / 4 in step
+// k, so a store instruction carries eight whole 64-byte runs -- 8 requests of two sectors instead of
+// 32 requests of 16 bytes to 32 lines.  Every warp that decodes tiles of one shape gets here at the
+// same unit; results do not depend on it: a lane of a partial warp, or of a warp whose lanes are
+// elsewhere (other tile shapes, row tails), stores its own run.
+__device__ __forceinline__ void s_flush(uint32_t stage, uint32_t lane, uint8_t* dst) {
+  if (s_whole_warp()) {
+#ifdef RSB200_EMU
+    ++g_emu_runs_shared;
+#endif
+    __syncwarp(); // the stages are written
+    const uint32_t lo = (uint32_t)reinterpret_cast<uintptr_t>(dst);
+    const uint32_t hi = (uint32_t)(reinterpret_cast<uintptr_t>(dst) >> 32);
+    const uint32_t c = lane & 3u;
+#pragma unroll 1
+    for (uint32_t k = 0; k < 4; ++k) {
+      const uint32_t src = 8u * k + (lane >> 2);
+      const uintptr_t d = ((uintptr_t)__shfl_sync(0xFFFFFFFFu, hi, (int)src) << 32) |
+                          __shfl_sync(0xFFFFFFFFu, lo, (int)src);
+      const uint4 v = lds_v4<0>(stage + S_STAGE * (src - lane) + s_stage_unit(src, c));
+      s_stg_v4(reinterpret_cast<uint8_t*>(d) + 16u * c, v);
+    }
+    __syncwarp(); // the stages are read before they are written again
+  } else {
+#ifdef RSB200_EMU
+    ++g_emu_runs_own;
+#endif
+#pragma unroll 1
+    for (uint32_t j = 0; j < 4; ++j)
+      s_stg_v4(dst + 16u * j, lds_v4<0>(stage + s_stage_unit(lane, j)));
+  }
 }
 
 __device__ __forceinline__ void s_prefetch_l2(const void* p) {
@@ -572,7 +648,7 @@ __device__ __forceinline__ void s_ldg_sector(const uint4* cb, uint32_t blk, uint
   b = s_ldg_l2_128b(cb + min(blk + 1u, bmax));
 }
 
-template <int G, bool WIDE>
+template <int G, bool WIDE, bool STAGED>
 __device__ __forceinline__ void
 stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp, const bool may_redo, const bool prefetch,
             const uint8_t* __restrict__ in, uint64_t in_total, uint8_t* __restrict__ out,
@@ -632,9 +708,22 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
   const uint32_t out_pitch = scp->out_pitch;
   uint8_t* orow = out + scp->out_offset + (uint64_t)scp->out_y * out_pitch + 2ull * scp->out_x;
   uint32_t bad_at = T_NOBAD, last_tl = 0;
-  // (WIDE: pairs of units leave together as one 32-byte sector where the rows allow it)
-  const bool wide = WIDE && ((reinterpret_cast<uintptr_t>(orow) | out_pitch) & 31u) == 0u;
+  // WIDE: the whole groups of 4 units of a row in front of store_w (<= row_samples) go through the
+  // stage, the rest directly.  (The small-launch form measured the same with the stage as without,
+  // and keeps direct stores: its registers spill less.)  A plan whose tables leave no room for the
+  // stage stores pairs of units as one 32-byte sector where the rows allow it.
+  static_assert(WIDE || !STAGED, "the stage is the full-launch form's");
+  const bool staged = STAGED;
+  const bool aligned32 = ((reinterpret_cast<uintptr_t>(orow) | out_pitch) & 31u) == 0u;
+  const bool pairs = WIDE && !staged && aligned32;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t stage = smem_u32(reinterpret_cast<const uint8_t*>(&sh) + stream_stage_offset(ntab_sh)) +
+                         S_STAGE * threadIdx.x;
+  const uint32_t groups = staged ? store_w >> 5 : 0u;
   uint32_t h0 = 0, h1 = 0, h2 = 0, h3 = 0;
+#ifndef RSB200_EMU
+  (void)aligned32;
+#endif
 
   for (uint32_t r = 0; r < rows; ++r) {
 #pragma unroll
@@ -731,15 +820,20 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
         f.nblk += 2u;
       }
       const uint32_t s = u << 3;
-      // two units = one 32-byte sector of the output row: the even unit waits in registers for the
-      // odd one and both leave back to back, so the sector is written whole at once (the plan
-      // picks WIDE by launch size)
-      if (WIDE && wide && !(u & 1u) && s + 16u <= store_w) {
+      if (WIDE && (u >> 2) < groups) {
+        sts_v4<0>(stage + s_stage_unit(lane, u), make_uint4(o0, o1, o2, o3));
+        if ((u & 3u) == 3u) {
+          s_flush(stage, lane, orow + 16ull * (u - 3u));
+#ifdef RSB200_EMU
+          g_emu_sector_stores += aligned32 ? 2u : 0u;
+#endif
+        }
+      } else if (pairs && !(u & 1u) && s + 16u <= store_w) { // the even unit waits for the odd one
         h0 = o0;
         h1 = o1;
         h2 = o2;
         h3 = o3;
-      } else if (WIDE && wide && (u & 1u) && s + 8u <= store_w) {
+      } else if (pairs && (u & 1u) && s + 8u <= store_w) {
         s_stg_sector(orow + 16ull * (u - 1u), h0, h1, h2, h3, o0, o1, o2, o3);
       } else if (s + 8 <= store_w) {
         s_stg_v4(orow + 16ull * u, make_uint4(o0, o1, o2, o3));
@@ -785,11 +879,10 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
 #undef S_SYM
 #undef S_SYMF
 
-#ifndef RSB200_S_LB
-#define RSB200_S_LB 6
-#endif
-// entry: one CTA of T_NT threads (the GPU kernel below; tests/emu replays it on the CPU)
-template <bool WIDE>
+// entry: one CTA of T_NT threads (the GPU kernel below; tests/emu replays it on the CPU).  STAGE: 1 =
+// the full-launch form with its output stage, 0 = without, -1 = whichever the plan's tables allow
+// (stream_staged).  The GPU launches a kernel per choice: a kernel holding both bodies spills more.
+template <bool WIDE, int STAGE = -1>
 __device__ __forceinline__ void
 stream_entry(StreamShared& sh, const uint8_t* __restrict__ in, uint64_t in_total,
              const DevScan* __restrict__ scans, const DevTable* __restrict__ tables, int ntab,
@@ -836,16 +929,25 @@ stream_entry(StreamShared& sh, const uint8_t* __restrict__ in, uint64_t in_total
   const DevScan* scp = scans + scan_idx;
   DevResult* res = results + scan_idx;
   const uint32_t G = scp->group;
-  if (G == 1)
-    stream_body<1, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, redo ? redo + id : nullptr);
-  else if (G == 2)
-    stream_body<2, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, redo ? redo + id : nullptr);
-  else
-    stream_body<4, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, redo ? redo + id : nullptr);
+  uint32_t* rd = redo ? redo + id : nullptr;
+  if (WIDE && (STAGE == 1 || (STAGE < 0 && stream_staged(ntab)))) {
+    if (G == 1)
+      stream_body<1, WIDE, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+    else if (G == 2)
+      stream_body<2, WIDE, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+    else
+      stream_body<4, WIDE, WIDE>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+  } else if (G == 1) {
+    stream_body<1, WIDE, false>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+  } else if (G == 2) {
+    stream_body<2, WIDE, false>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+  } else {
+    stream_body<4, WIDE, false>(sh, ntab, scp, may_redo, prefetch, in, in_total, out, res, rd);
+  }
 }
 
 #ifndef RSB200_EMU
-template <bool WIDE>
+template <bool WIDE, bool STAGED>
 __global__ void __launch_bounds__(T_NT, RSB200_S_LB)
     k2_stream_kernel(const uint8_t* __restrict__ in, uint64_t in_total, const DevScan* __restrict__ scans,
                      const DevTable* __restrict__ tables, int ntab, uint8_t* __restrict__ out,
@@ -853,7 +955,9 @@ __global__ void __launch_bounds__(T_NT, RSB200_S_LB)
                      uint32_t nids, uint32_t* __restrict__ redo, int prefetch) {
   extern __shared__ __align__(128) uint8_t s_smem_raw[];
   StreamShared& sh = *reinterpret_cast<StreamShared*>(s_smem_raw);
-  stream_entry<WIDE>(sh, in, in_total, scans, tables, ntab, out, results, scan_ids, nids, redo, prefetch != 0);
+  static_assert(WIDE || !STAGED, "the stage is the full-launch form's");
+  stream_entry<WIDE, STAGED ? 1 : 0>(sh, in, in_total, scans, tables, ntab, out, results, scan_ids, nids, redo,
+                                     prefetch != 0);
 }
 #endif
 

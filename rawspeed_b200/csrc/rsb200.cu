@@ -1801,13 +1801,14 @@ constexpr uint32_t BIG_SEGMENT_BYTES = 256u << 10; // above this a segment gets 
 #define RSB200_STREAM_DEFAULT 1
 #endif
 // k2_stream_kernel: an L2 prefetch ahead of every sector is meant for launches too small to fill the
-// machine (latency bound) and left out of full ones (it adds requests); the split, like the WIDE form of the
-// full launches (a pair of units leaves as two back-to-back 128-bit stores), has not been measured on H100
+// machine (latency bound) and left out of full ones (it adds requests); the split has not been measured on
+// H100.  The full launches stage their output in shared memory and store it in 64-byte runs (DESIGN.md, K2S)
 constexpr size_t K2P_MAX_SEGMENTS = 0; // (k2_par_kernel: off by default until measured; RSB200_PAR_MAX / RSB200_LJPEG_PATH=par)
 // half a wave: for sm_90a ptxas gives k2_stream_kernel 80 registers, so 6 CTAs of 128 threads fit an SM
 constexpr int K2S_PREFETCH_CTAS_PER_SM = 3;
-// k2_stream_kernel<true> (no prefetch, whole-sector stores) for launches of more than half a wave of
-// thread-path segments, k2_stream_kernel<false> up to that; RSB200_STREAM_FORM overrides it
+// k2_stream_kernel<true, *> (no prefetch; output staged where the tables leave room, else pairs of units
+// stored as whole sectors) for launches of more than half a wave of thread-path segments,
+// k2_stream_kernel<false, false> up to that; RSB200_STREAM_FORM overrides it
 static bool stream_full_launch(const rsb200_ctx* ctx, const rsb200_plan* p) {
   if (p->stream_form)
     return p->stream_form == 2;
@@ -2728,13 +2729,20 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
     }
     if (p->nthread && p->use_stream) {
       // small launches are latency bound (L2 prefetch ahead, 128-bit stores), full ones are bound
-      // by the number of memory requests (no prefetch, whole-sector stores)
+      // by the number of memory requests (no prefetch, output stored in 64-byte runs)
+      // (the output stage where the plan's tables leave room for it, see stream_staged)
+      const int nb = (p->nthread + T_NT - 1) / T_NT;
+      const size_t smem = stream_smem_bytes(p->ntables);
       if (!stream_full_launch(ctx, p))
-        k2_stream_kernel<false><<<(p->nthread + T_NT - 1) / T_NT, T_NT, stream_smem_bytes(p->ntables), st>>>(
+        k2_stream_kernel<false, false><<<nb, T_NT, smem, st>>>(
             in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
             p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 1);
+      else if (stream_staged(p->ntables))
+        k2_stream_kernel<true, true><<<nb, T_NT, smem, st>>>(
+            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
+            p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 0);
       else
-        k2_stream_kernel<true><<<(p->nthread + T_NT - 1) / T_NT, T_NT, stream_smem_bytes(p->ntables), st>>>(
+        k2_stream_kernel<true, false><<<nb, T_NT, smem, st>>>(
             in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
             p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 0);
       CUDA_TRY(ctx, cudaGetLastError());
