@@ -576,6 +576,37 @@ int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* jobs, int nj
                             rsb200_plan** plan);
 
 /* ------------------------------------------------------------------ */
+/* Samsung SRW V1, compression 32772 (SURVEY 8(f)4).                     */
+/*   SamsungV1Decompressor::decompress                                   */
+/*   decompressors/SamsungV1Decompressor.cpp:81-140                      */
+/*   (plain MSB bit stream, fixed prefix code, per-parity left predictor,*/
+/*   rows start from two rows up; every value must stay in 0..4095).     */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint64_t in_offset; /* first byte of the stream                                 */
+  uint32_t in_size;   /* bytes available; < 2^28                                  */
+  uint32_t bits;      /* the container's bits per sample (must be 12)            */
+  int32_t width;      /* multiple of 32, 32..5664, and height (even, 2..3714):    */
+  int32_t height;     /* the constructor's checks, SamsungV1Decompressor.cpp:52-60 */
+  uint64_t out_offset; /* byte offset of image row 0; multiple of 4               */
+  uint32_t out_pitch;  /* bytes; multiple of 4, >= 2 * width                     */
+  uint32_t reserved;   /* 0                                                      */
+} rsb200_samsung1_job;
+
+/* A bit count other than 12 or dimensions the reference's constructor rejects fail
+ * plan creation with RSB200_ERR_RDE ("Unexpected bit per pixel" / "Unexpected image
+ * dimensions found"); an out_offset or out_pitch that is not a multiple of 4, a pitch
+ * below 2 * width, in_size >= 2^28 or a non-zero reserved field with RSB200_ERR_ARG.
+ * rsb200_plan_results() per job: RSB200_ERR_RDE with consumed == RSB200_PENTAX_OOB |
+ * (row << 14) | col = "decoded value out of bounds" at the first pixel (row-major)
+ * whose value left 0..4095; RSB200_ERR_IOE with consumed == (row << 14) | col of the
+ * pixel whose refill started more than 8 bytes behind the stream (0 for a stream of
+ * fewer than 4 bytes), when it comes first.  Pixels before the error are written; the
+ * rest of the image is left as it was. */
+int rsb200_samsung1_plan_create(rsb200_ctx* ctx, const rsb200_samsung1_job* jobs, int njobs,
+                                rsb200_plan** plan);
+
+/* ------------------------------------------------------------------ */
 /* Nikon NEF Huffman codec without split (SURVEY 8(f)2).                 */
 /*   NikonDecompressor::decompress  decompressors/NikonDecompressor.cpp:513-560 */
 /*   (plain MSB bit stream, nikon_tree table, per-parity left predictor, */

@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -367,6 +367,14 @@ def arw1_plan(ctx, jobs):
     ja = (Arw1Job * len(jobs))(*jobs)
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_arw1_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def samsung1_plan(ctx, jobs):
+    """Samsung SRW V1 streams (SamsungV1Decompressor::decompress), one job per frame."""
+    ja = (SamsungV1Job * len(jobs))(*jobs)
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_samsung1_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

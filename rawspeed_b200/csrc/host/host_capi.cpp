@@ -352,6 +352,22 @@ int rsb200h_samsung_v0(uint16_t* img_data, int w, int h, int pitch, const uint8_
   });
 }
 
+// cpp: components per pixel of the image (the constructor refuses anything but 1)
+int rsb200h_samsung_v1(uint16_t* img_data, int w, int h, int cpp, int pitch, const uint8_t* data,
+                       uint32_t size, int bit, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, cpp, pitch, true, 1, 1);
+    SamsungV1Decompressor d(img, ByteStream(data, size), bit);
+    try {
+      d.decompress();
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
                                  uint32_t size, rsb200h_err* e) {
   return guarded(e, [&] {

@@ -814,6 +814,47 @@ void SamsungV0Decompressor::decompress() const {
   }
 }
 
+// ------------------------------------------------------------------ Samsung V1
+SamsungV1Decompressor::SamsungV1Decompressor(const RawImage& image, ByteStream bs_, int bit)
+    : mRaw(image), bs(bs_) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||
+      mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  if (bit != 12)
+    ThrowRDE("Unexpected bit per pixel (%d)", bit);
+  const uint32_t w = mRaw->dim.x;
+  const uint32_t h = mRaw->dim.y;
+  if (w == 0 || h == 0 || w % 32 != 0 || h % 2 != 0 || w > 5664 || h > 3714)
+    ThrowRDE("Unexpected image dimensions found: (%u; %u)", w, h);
+}
+
+void SamsungV1Decompressor::decompress() const {
+  if (bs.getRemainSize() < 4) // BitStreamerMSB ctor (BitStreamer.h:56-60)
+    ThrowIOE("Bit stream size is smaller than MaxProcessBytes");
+  rsb200_samsung1_job job;
+  std::memset(&job, 0, sizeof job);
+  job.in_offset = 0;
+  job.in_size = bs.getRemainSize();
+  job.bits = 12;
+  job.width = mRaw->dim.x;
+  job.height = mRaw->dim.y;
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  PlanGuard pg;
+  engineCheck(rsb200_samsung1_plan_create(engine(), &job, 1, &pg.p), "rsb200_samsung1_plan_create");
+  RawImage img = mRaw;
+  runOnImage(pg.p, bs.begin() + bs.getPosition(), bs.getRemainSize(), img, /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  if (res.status == RSB200_ERR_RDE)
+    ThrowRDE("decoded value out of bounds"); // SamsungV1Decompressor.cpp:135-136
+  if (res.status == RSB200_ERR_IOE)
+    ThrowIOE("Buffer overflow read in BitStreamer");
+  engineCheck(rc, "rsb200_plan_results");
+}
+
 // ------------------------------------------------------------------ Sony ARW1
 SonyArw1Decompressor::SonyArw1Decompressor(RawImage img) : mRaw(std::move(img)) {
   if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||

@@ -597,6 +597,20 @@ private:
   std::vector<ByteStream> stripes;
 };
 
+// ---------------------------------------------------------------- Samsung V1
+// decompressors/SamsungV1Decompressor.h: same constructor (image, stream, bits per sample; its
+// checks, SamsungV1Decompressor.cpp:45-61) and decompress().  The whole decode runs on the device
+// (samsung1.cuh); errors are thrown with the reference's classes and messages.
+class SamsungV1Decompressor final {
+public:
+  SamsungV1Decompressor(const RawImage& image, ByteStream bs, int bit);
+  void decompress() const;
+
+private:
+  RawImage mRaw;
+  ByteStream bs;
+};
+
 // ---------------------------------------------------------------- Sony ARW1
 // decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
 // SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs

@@ -669,8 +669,10 @@ __device__ __forceinline__ FSync f_sync(FusedShared& sh, uint32_t sb, const Fuse
     uint32_t my_phase = (tid == 0) ? (cy.sym % G) : 0u;
     // arw1_align: 1 = the guesses of threads 1.., 2 = thread 0's start too (a range's halo chunk);
     // they stay guesses: the fixed point below is exact
+    // (Samsung V1, DevScan::kind 5: the same with samsung1_run_phase, ljpeg_types.h)
     if (arw1_align > (tid == 0 ? 1u : 0u) && active) // (thread 0: cy.pos == sub_lo == 0 then)
-      my_start += arw1_run_phase(sh.ub[sub_lo >> 5], sh.ub[(sub_lo >> 5) + 1]);
+      my_start += sh.sc.kind == 5 ? samsung1_run_phase(sh.ub[sub_lo >> 5], sh.ub[(sub_lo >> 5) + 1])
+                                  : arw1_run_phase(sh.ub[sub_lo >> 5], sh.ub[(sub_lo >> 5) + 1]);
     const uint32_t start0 = my_start; // thread 0's start (cy.pos unless aligned)
     if (!active)
       my_start = 0xFFFFFFF0u;

@@ -137,13 +137,14 @@ __device__ __forceinline__ void r_stream(const FusedShared& sh, const uint8_t* i
 // reference decodes codes that start there as long as the refill before them is allowed
 // (plain_overread): at the end of the segment, symbols that start up to 8 bytes behind the last
 // data byte are parsed too (ub holds 16 zero bytes behind the data).  The plain pump only comes
-// with one table (Pentax, Nikon): MULTI instantiations are plain f_unstuff.
+// with one table (Pentax, Nikon): MULTI instantiations are plain f_unstuff.  Samsung V1 refills to
+// 23 bits, not 32, before a symbol (samsung1.cuh): its symbols start up to 8 bytes + 9 bits behind.
 template <bool MULTI>
 __device__ __forceinline__ FChunk r_unstuff(FusedShared& sh, FStream& st, const FusedCarry& cy,
                                             uint32_t chunk) {
   FChunk co = f_unstuff(sh, st, cy, chunk);
   if (!MULTI && st.plain && co.final_chunk && st.limit == st.skew + sh.sc.in_size)
-    co.end_all += 8u * 8u + 1u;
+    co.end_all += 8u * 8u + (sh.sc.kind == 5 ? 10u : 1u);
   return co;
 }
 
@@ -183,9 +184,10 @@ __device__ __forceinline__ void range_count_body(FusedShared& sh, const uint8_t*
     mbar_wait(&sh.bar, (chunk - c_first) & 1u);
     st.pending = false;
     const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
-    // ARW1: every speculative start follows a run of zero differences, including this CTA's guess at
-    // the start of its halo chunk
-    const uint32_t align = (!MULTI && sh.sc.kind == 4) ? ((chunk == c_first && r > 0) ? 2u : 1u) : 0u;
+    // ARW1 and Samsung V1: every speculative start follows a run of zero differences, including this
+    // CTA's guess at the start of its halo chunk
+    const uint32_t align =
+        (!MULTI && (sh.sc.kind == 4 || sh.sc.kind == 5)) ? ((chunk == c_first && r > 0) ? 2u : 1u) : 0u;
     const FSync so = f_sync<MULTI>(sh, sb, cy, co, G, align);
     uint32_t total_syms;
     (void)f_block_scan(so.d.count, sh.warp_tmp[3], &total_syms);
@@ -414,7 +416,8 @@ __device__ __forceinline__ void range_diffs_body(FusedShared& sh, const uint8_t*
     mbar_wait(&sh.bar, (chunk - c_own0) & 1u);
     st.pending = false;
     const FChunk co = r_unstuff<MULTI>(sh, st, cy, chunk);
-    const FSync so = f_sync<MULTI>(sh, sb, cy, co, G, (!MULTI && sh.sc.kind == 4) ? 1u : 0u);
+    const FSync so =
+        f_sync<MULTI>(sh, sb, cy, co, G, (!MULTI && (sh.sc.kind == 4 || sh.sc.kind == 5)) ? 1u : 0u);
     const FSub d = so.d;
     uint32_t total_syms;
     const uint32_t sincl = f_block_scan(d.count, sh.warp_tmp[3], &total_syms);

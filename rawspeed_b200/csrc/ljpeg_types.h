@@ -40,7 +40,8 @@ struct DevScan {
   uint8_t group;        // samples per MCU / CR2 group
   uint8_t ncomp;
   uint8_t multi_table;  // components use different tables -> phase matters
-  uint8_t kind;         // 0 = LJPEG tile, 1 = CR2, 2 = Pentax (K3P reconstruction)
+  uint8_t kind;         // 0 = LJPEG tile, 1 = CR2, 2 = Pentax (K3P reconstruction), 3 = Nikon,
+                        // 4 = Sony ARW1 (arw1.cuh), 5 = Samsung V1 (samsung1.cuh)
   uint8_t table_of[12]; // slot (0..3) of the block-local table of sample p
   uint8_t pattern;      // component pattern of a group (PAT_*)
   uint8_t pump;         // 0 = JPEG bit source (FF00 stuffing, FFxx ends the data);
@@ -105,6 +106,17 @@ RSB_LJ_HD inline SymLen decode_sym(const DevTable*  t,
     s.total = 1;
   }
   return s;
+}
+
+// Samsung V1 (samsung1.cuh): a zero difference is the code 110100.  A parse that starts on any of
+// the 5 wrong residues inside a run of them falls into a cycle of the residues 2 and 4 mod 6 and
+// never resynchronises, so speculative starts inside such a run are moved to its phase (f_sync's
+// run alignment): the offset 0..5 at which the 32 bits of x0:x1 are 110100 repeated, else 0.
+RSB_LJ_HD inline uint32_t samsung1_run_phase(uint32_t x0, uint32_t x1) {
+  for (uint32_t o = 0; o < 6; ++o)
+    if (((x0 << o) | (o ? x1 >> (32 - o) : 0u)) == 0xD34D34D3u)
+      return o;
+  return 0;
 }
 
 // AbstractPrefixCodeDecoder::processSymbol + extend

@@ -30,6 +30,7 @@
 #include "nikon.cuh"
 #include "arw1.cuh"
 #include "samsung0.cuh"
+#include "samsung1.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -374,6 +375,15 @@ struct rsb200_plan {
   int2* d_arw1_runpre = nullptr;
   Arw1Info* d_arw1_info = nullptr;
   uint32_t arw1_max_runs = 0, arw1_max_tiles = 0, arw1_max_words = 0;
+  // Samsung V1 frames (DevScan::kind == 5, samsung1.cuh): reconstruction and end-of-stream scratch
+  bool has_samsung1 = false;
+  int ns1 = 0;
+  DevS1* d_s1 = nullptr;
+  uint16_t* d_s1_colvals = nullptr; // 2 per row
+  uint2* d_s1_rowbits = nullptr;    // per row
+  uint32_t* d_s1_oob = nullptr;     // per frame: first out-of-range pixel
+  uint32_t* d_s1_lim = nullptr;     // per frame: first pixel not written
+  uint32_t s1_max_h = 0;
   cudaStream_t last_stream = nullptr;
   bool ran = false;
 };
@@ -1830,6 +1840,9 @@ static bool par_eligible(const DevScan& d) {
   return thread_eligible(d) && !d.multi_table && d.n_samples >= 8 && d.in_size >= 8;
 }
 
+static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
+                                    const std::vector<DevTable>& ht, ScanBuild& b);
+
 static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
                              const rsb200_huff_table* tables, int ntables, ScanBuild& b,
                              bool /*unused*/) {
@@ -1839,6 +1852,13 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
       delete p;
       return set_err(ctx, RSB200_ERR_ARG, "huffman table %d is malformed", i);
     }
+  return finish_ljpeg_plan_tables(ctx, p, ht, b);
+}
+
+// the rest of finish_ljpeg_plan, for plans whose device tables are built by their codec
+static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
+                                    const std::vector<DevTable>& ht, ScanBuild& b) {
+  const int ntables = (int)ht.size();
   p->kind = 1;
   p->ntab_slots = 1;
   for (const DevScan& d : b.scans)
@@ -1940,7 +1960,9 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
     const bool is_big = d.kind != 0 || d.in_size > BIG_SEGMENT_BYTES;
     if (is_big)
       (d.kind == 2 ? p->has_pentax
-                   : (d.kind == 3 ? p->has_nikon : (d.kind == 4 ? p->has_arw1 : p->has_k3))) = true;
+                   : (d.kind == 3 ? p->has_nikon
+                                  : (d.kind == 4 ? p->has_arw1
+                                                 : (d.kind == 5 ? p->has_samsung1 : p->has_k3)))) = true;
     if (!is_big) {
       if (use_thread && (p->use_par ? par_eligible(d) : thread_eligible(d))) {
         thread_ids.push_back((uint32_t)i);
@@ -1966,7 +1988,7 @@ static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
     d.col_offset = b.col_elems;
     b.col_elems += (uint64_t)d.rows * 4;
     d.row_begin = (uint32_t)b.rows.size();
-    for (uint32_t r = 0; d.kind != 4 && r < d.rows; ++r) // (ARW1: arw1.cuh reconstructs)
+    for (uint32_t r = 0; d.kind < 4 && r < d.rows; ++r) // (ARW1, Samsung V1: their own kernels)
       b.rows.push_back(K3RowRef{(uint32_t)i, r});
     const uint32_t skew = (uint32_t)(d.in_offset & 15ull);
     const uint32_t range_bytes = (uint32_t)R_CHUNKS * F_RAW;
@@ -2320,6 +2342,110 @@ extern "C" int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* j
   if (e != cudaSuccess) {
     rsb200_plan_destroy(p);
     return set_err(ctx, RSB200_ERR_CUDA, "arw1 plan allocation failed: %s", cudaGetErrorString(e));
+  }
+  p->launches_per_run += 4;
+  *out = p;
+  return RSB200_OK;
+}
+
+// ------------------------------------------------------------------
+// Samsung V1: one plain-MSB stream per frame (K2R with the LUT-only table, samsung1.cuh)
+// ------------------------------------------------------------------
+extern "C" int rsb200_samsung1_plan_create(rsb200_ctx* ctx, const rsb200_samsung1_job* jobs,
+                                           int njobs, rsb200_plan** out) {
+  if (!ctx || !jobs || njobs <= 0 || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "samsung1_plan_create: bad arguments");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung1_job& j = jobs[i];
+    // SamsungV1Decompressor ctor (SamsungV1Decompressor.cpp:52-60)
+    if (j.bits != 12)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected bit per pixel (%d)", i, (int)j.bits);
+    if (j.width <= 0 || j.height <= 0 || j.width % 32 != 0 || j.height % 2 != 0 || j.width > 5664 ||
+        j.height > 3714)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected image dimensions found: (%u; %u)", i,
+                     (unsigned)j.width, (unsigned)j.height);
+    // the stores write two pixels as one 32-bit word
+    if (j.in_size >= (1u << 28) || (uint64_t)j.width * 2 > j.out_pitch || (j.out_offset % 4) ||
+        (j.out_pitch % 4) || j.reserved)
+      return set_err(ctx, RSB200_ERR_ARG, "samsung1 job %d: malformed descriptor", i);
+  }
+  rsb200_plan* p = new (std::nothrow) rsb200_plan();
+  if (!p)
+    return RSB200_ERR_CUDA;
+  p->ctx = ctx;
+  ScanBuild b;
+  std::vector<DevS1> fr((size_t)njobs);
+  uint64_t rows = 0;
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung1_job& j = jobs[i];
+    const uint32_t w = (uint32_t)j.width, h = (uint32_t)j.height;
+    DevS1& f = fr[(size_t)i];
+    memset(&f, 0, sizeof f);
+    f.w = w;
+    f.h = h;
+    f.out_offset = j.out_offset;
+    f.out_pitch = j.out_pitch;
+    f.tstar = samsung1_tstar(j.in_size);
+    f.scan = (uint32_t)i;
+    f.row_base = (uint32_t)rows;
+    rows += h;
+    p->s1_max_h = std::max(p->s1_max_h, h);
+    DevScan d;
+    memset(&d, 0, sizeof d);
+    d.in_offset = j.in_offset;
+    d.in_size = j.in_size;
+    d.row_samples = w;
+    d.rows = h;
+    d.n_samples = w * h;
+    d.group = 1;
+    d.ncomp = 1;
+    d.kind = 5;
+    d.pump = 1;
+    d.pattern = PAT_PLAIN;
+    const uint8_t tab[4] = {0, 0, 0, 0};
+    const uint8_t comp_of_pos[1] = {0};
+    assign_tables(d, tab, 1, comp_of_pos, 1);
+    d.out_offset = j.out_offset;
+    d.out_pitch = j.out_pitch;
+    d.mcu_w = 1;
+    d.mcu_h = 1;
+    d.store_w = w;
+    b.scans.push_back(d);
+    p->in_bytes += j.in_size;
+    p->out_bytes += (uint64_t)w * h * 2;
+    p->pixels += (uint64_t)w * h;
+    p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
+    p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)h - 1) * j.out_pitch + 2ull * w));
+  }
+  // (the row kernels' 1-D grids: one CTA per 8 rows of the tallest frame, per frame)
+  if (rows >= (1ull << 31) ||
+      (uint64_t)njobs * ((p->s1_max_h + S1_ROWS_PER_CTA - 1) / S1_ROWS_PER_CTA) >= (1ull << 31)) {
+    delete p;
+    return set_err(ctx, RSB200_ERR_ARG, "samsung1 plan: too many frames for one plan");
+  }
+  std::vector<DevTable> ht(1);
+  samsung1_dev_table(ht[0]);
+  int rc = finish_ljpeg_plan_tables(ctx, p, ht, b);
+  if (rc != RSB200_OK)
+    return rc;
+  for (size_t i = 0; i < fr.size(); ++i)
+    fr[i].diff_offset = b.scans[i].diff_offset;
+  p->ns1 = njobs;
+  cudaError_t e = rsb_dev_alloc((void**)&p->d_s1, sizeof(DevS1) * fr.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_s1, fr.data(), sizeof(DevS1) * fr.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_s1_colvals, sizeof(uint16_t) * 2 * rows);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_s1_rowbits, sizeof(uint2) * rows);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_s1_oob, sizeof(uint32_t) * fr.size());
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc((void**)&p->d_s1_lim, sizeof(uint32_t) * fr.size());
+  if (e != cudaSuccess) {
+    rsb200_plan_destroy(p);
+    return set_err(ctx, RSB200_ERR_CUDA, "samsung1 plan allocation failed: %s", cudaGetErrorString(e));
   }
   p->launches_per_run += 4;
   *out = p;
@@ -2839,6 +2965,20 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
                                                             p->d_arw1_info, p->d_results);
         arw1_apply_kernel<<<dim3(p->arw1_max_tiles, p->narw1), ARW1_NT, 0, st>>>(
             p->d_arw1, p->d_diffs, p->d_arw1_runpre, p->d_arw1_info, outp, p->d_results);
+        nk3 += 4;
+      }
+      if (p->has_samsung1) {
+        CUDA_TRY(ctx, cudaMemsetAsync(p->d_s1_oob, 0xFF, sizeof(uint32_t) * (size_t)p->ns1, st));
+        const uint32_t rb = (p->s1_max_h + S1_ROWS_PER_CTA - 1) / S1_ROWS_PER_CTA;
+        const uint32_t rows_grid = rb * (uint32_t)p->ns1; // (< 2^31: checked at plan creation)
+        s1_column_kernel<<<(p->ns1 * 4 * 32 + 127) / 128, 128, 0, st>>>(p->d_s1, p->ns1, p->d_diffs,
+                                                                        p->d_s1_colvals, p->d_s1_oob);
+        s1_row_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1, rb, p->d_diffs, p->d_s1_colvals,
+                                                   p->d_s1_rowbits, p->d_s1_oob);
+        s1_scan_kernel<<<p->ns1, S1_SCAN_NT, 0, st>>>(p->d_s1, p->d_diffs, p->d_s1_rowbits,
+                                                      p->d_s1_oob, p->d_s1_lim, p->d_results);
+        s1_store_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1, rb, p->d_diffs, p->d_s1_colvals,
+                                                     p->d_s1_lim, outp);
         nk3 += 4;
       }
       CUDA_TRY(ctx, cudaGetLastError());
@@ -3554,6 +3694,18 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
       results[i].status = p->h_results[i].status;
       results[i].consumed = p->h_results[i].consumed;
     }
+    if (first == RSB200_OK && p->h_results[i].status != 0 && p->has_samsung1) {
+      // SamsungV1Decompressor.cpp:135-136 / BitStreamer.h:58-59, 125-127
+      first = (int)p->h_results[i].status;
+      if (first == RSB200_ERR_RDE)
+        set_err(ctx, first, "job %d: decoded value out of bounds (col %u, row %u)", i,
+                p->h_results[i].consumed & 0x3FFFu, (p->h_results[i].consumed >> 14) & 0xFFFu);
+      else if (p->h_results[i].consumed == 0) // (T* >= 106 for 4 bytes and more: only a short stream)
+        set_err(ctx, first, "job %d: Bit stream size is smaller than MaxProcessBytes", i);
+      else
+        set_err(ctx, first, "job %d: Buffer overflow read in BitStreamer (col %u, row %u)", i,
+                p->h_results[i].consumed & 0x3FFFu, p->h_results[i].consumed >> 14);
+    }
     if (first == RSB200_OK && p->h_results[i].status != 0 && p->has_arw1) {
       // SonyArw1Decompressor.cpp:86-87 / BitStreamer.h:100-131
       first = (int)p->h_results[i].status;
@@ -3773,6 +3925,11 @@ extern "C" void rsb200_plan_destroy(rsb200_plan* p) {
   rsb_dev_free(p->d_arw1_lastoff);
   rsb_dev_free(p->d_arw1_runpre);
   rsb_dev_free(p->d_arw1_info);
+  rsb_dev_free(p->d_s1);
+  rsb_dev_free(p->d_s1_colvals);
+  rsb_dev_free(p->d_s1_rowbits);
+  rsb_dev_free(p->d_s1_oob);
+  rsb_dev_free(p->d_s1_lim);
   if (p->h_oob)
     rsb_host_free(p->h_oob);
   if (p->h_results)
