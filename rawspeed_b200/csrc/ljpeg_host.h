@@ -8,6 +8,8 @@
 
 #include <algorithm>
 #include <cstring>
+#include <tuple>
+#include <vector>
 
 namespace rsb200 {
 
@@ -124,6 +126,26 @@ inline void tile_params(const DevScan& d, int npiece_max, int dcap, int preroll_
   if (preroll_override >= 0)
     pre = (uint32_t)preroll_override;
   preroll = pre;
+}
+
+// Order of the thread path's segments (one per thread, a warp takes 32 consecutive ones).  The lanes of
+// a warp flush k2_stream_kernel's output stage together only where they are at the same row and unit of
+// the same kernel body, so a warp should hold segments that agree on everything that steers it: the
+// group G (one body per G), row_samples (units per row), rows and store_w (staged groups per row).
+// Segments of one such shape form a class; classes run by descending samples per segment, then by
+// descending stored width (the short edge tiles last), and a class keeps the input order (in scan order
+// a warp of interior tiles is one tile row of a frame: neighbouring input and output).  Returns the
+// positions in `ids` in that order.
+inline std::vector<uint32_t> thread_shape_order(const DevScan* scans, const std::vector<uint32_t>& ids) {
+  std::vector<uint32_t> perm(ids.size());
+  for (size_t k = 0; k < ids.size(); ++k)
+    perm[k] = (uint32_t)k;
+  auto key = [&](uint32_t k) {
+    const DevScan& d = scans[ids[k]];
+    return std::make_tuple(~((uint64_t)d.rows * d.row_samples), ~d.store_w, d.group, d.row_samples, d.rows);
+  };
+  std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) { return key(a) < key(b); });
+  return perm;
 }
 
 // C-ABI scan -> device descriptor (validation included); false = malformed

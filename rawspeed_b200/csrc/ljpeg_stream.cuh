@@ -569,17 +569,27 @@ __device__ __forceinline__ void s_stg_sector(void* p, uint32_t a, uint32_t b, ui
   s_stg_v4(static_cast<uint8_t*>(p) + 16, make_uint4(e, f, g, h));
 }
 
-// "every lane of my warp is here" -- a hint only: results do not depend on it (s_flush)
+// "every lane of my warp is here" -- a hint only: results do not depend on it (s_flush).  `at` names the
+// flush (G, row, unit): lanes meet only at the same one, the GPU's lanes at the same program point.
 #ifdef RSB200_EMU
 inline unsigned long long g_emu_runs_shared = 0; // (CPU replay: 64-byte runs stored by the whole warp)
 inline unsigned long long g_emu_runs_own = 0;    // (... by the lane whose run it is)
-// a replay that gathers the lanes of a warp defines this; otherwise every lane is alone
+// a replay that gathers the lanes of a warp defines one of these: RSB200_EMU_WHOLE_WARP_AT(at) where the
+// place of the flush matters to it, RSB200_EMU_WHOLE_WARP() where it does not; otherwise every lane is alone
 #ifndef RSB200_EMU_WHOLE_WARP
 #define RSB200_EMU_WHOLE_WARP() false
 #endif
-__device__ __forceinline__ bool s_whole_warp() { return RSB200_EMU_WHOLE_WARP(); }
+#ifndef RSB200_EMU_WHOLE_WARP_AT
+#define RSB200_EMU_WHOLE_WARP_AT(at) ((void)(at), RSB200_EMU_WHOLE_WARP())
+#endif
+__device__ __forceinline__ bool s_whole_warp(uint64_t at) { return RSB200_EMU_WHOLE_WARP_AT(at); }
 #else
-__device__ __forceinline__ bool s_whole_warp() { return __activemask() == 0xFFFFFFFFu; }
+__device__ __forceinline__ bool s_whole_warp(uint64_t) { return __activemask() == 0xFFFFFFFFu; }
+#endif
+#if defined(RSB200_FLUSH_COUNT) && !defined(RSB200_EMU)
+// profiling builds only (-DRSB200_FLUSH_COUNT, tools/flush_count.py): 64-byte runs stored by whole warps
+// [0] and by single lanes [1], read by rsb200_debug_flush_runs
+__device__ unsigned long long g_flush_runs[2];
 #endif
 // The lane's last four units (its stage) go to `dst` (16-byte aligned).  Where the whole warp is here,
 // the lanes store each other's stages: lane l writes 16 bytes of the run of lane 8k + l / 4 in step
@@ -587,10 +597,13 @@ __device__ __forceinline__ bool s_whole_warp() { return __activemask() == 0xFFFF
 // 32 requests of 16 bytes to 32 lines.  Every warp that decodes tiles of one shape gets here at the
 // same unit; results do not depend on it: a lane of a partial warp, or of a warp whose lanes are
 // elsewhere (other tile shapes, row tails), stores its own run.
-__device__ __forceinline__ void s_flush(uint32_t stage, uint32_t lane, uint8_t* dst) {
-  if (s_whole_warp()) {
+__device__ __forceinline__ void s_flush(uint32_t stage, uint32_t lane, uint8_t* dst, uint64_t at) {
+  if (s_whole_warp(at)) {
 #ifdef RSB200_EMU
     ++g_emu_runs_shared;
+#elif defined(RSB200_FLUSH_COUNT)
+    if (lane == 0u)
+      atomicAdd(&g_flush_runs[0], 32ull);
 #endif
     __syncwarp(); // the stages are written
     const uint32_t lo = (uint32_t)reinterpret_cast<uintptr_t>(dst);
@@ -608,6 +621,12 @@ __device__ __forceinline__ void s_flush(uint32_t stage, uint32_t lane, uint8_t* 
   } else {
 #ifdef RSB200_EMU
     ++g_emu_runs_own;
+#elif defined(RSB200_FLUSH_COUNT)
+    {
+      const uint32_t m = __activemask();
+      if (lane == (uint32_t)(__ffs(m) - 1))
+        atomicAdd(&g_flush_runs[1], (unsigned long long)__popc(m));
+    }
 #endif
 #pragma unroll 1
     for (uint32_t j = 0; j < 4; ++j)
@@ -823,7 +842,7 @@ stream_body(StreamShared& sh, const int ntab_sh, const DevScan* __restrict__ scp
       if (WIDE && (u >> 2) < groups) {
         sts_v4<0>(stage + s_stage_unit(lane, u), make_uint4(o0, o1, o2, o3));
         if ((u & 3u) == 3u) {
-          s_flush(stage, lane, orow + 16ull * (u - 3u));
+          s_flush(stage, lane, orow + 16ull * (u - 3u), ((uint64_t)r << 32) | (u << 3) | (uint32_t)G);
 #ifdef RSB200_EMU
           g_emu_sector_stores += aligned32 ? 2u : 0u;
 #endif

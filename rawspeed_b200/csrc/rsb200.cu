@@ -499,6 +499,22 @@ extern "C" int rsb200_debug_tile_phase_cycles(unsigned long long* out16, int res
 }
 #endif
 
+#ifdef RSB200_FLUSH_COUNT
+// profiling builds only (tools/flush_count.py): read/reset the 64-byte runs k2_stream_kernel's output
+// stage stored by whole warps (out2[0]) and by single lanes (out2[1])
+extern "C" int rsb200_debug_flush_runs(unsigned long long* out2, int reset) {
+  cudaDeviceSynchronize();
+  if (out2 && cudaMemcpyFromSymbol(out2, rsb200::g_flush_runs, 2 * sizeof(unsigned long long)) != cudaSuccess)
+    return RSB200_ERR_CUDA;
+  if (reset) {
+    unsigned long long z[2] = {0, 0};
+    if (cudaMemcpyToSymbol(rsb200::g_flush_runs, z, sizeof z) != cudaSuccess)
+      return RSB200_ERR_CUDA;
+  }
+  return RSB200_OK;
+}
+#endif
+
 // ------------------------------------------------------------------
 // unpack plan
 // ------------------------------------------------------------------
@@ -2054,6 +2070,17 @@ static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
       build_groups(tile_ids);
       p->host_tiles_only = true;
     }
+  }
+  // The thread path decodes its segments by shape (thread_shape_order), so that whole warps flush the
+  // output stage together.  Everything below that is indexed by position (the ids with their bit 31,
+  // the per-thread scratch, the redo flags and parameters) is built in this order; the host-buffer
+  // groups above keep scan order.
+  {
+    const std::vector<uint32_t> perm = thread_shape_order(b.scans.data(), thread_ids);
+    std::vector<uint32_t> ordered(perm.size());
+    for (size_t k = 0; k < perm.size(); ++k)
+      ordered[k] = thread_ids[perm[k]];
+    thread_ids.swap(ordered);
   }
   p->h_in_size.resize(b.scans.size());
   for (size_t i = 0; i < b.scans.size(); ++i)
