@@ -607,6 +607,50 @@ int rsb200_samsung1_plan_create(rsb200_ctx* ctx, const rsb200_samsung1_job* jobs
                                 rsb200_plan** plan);
 
 /* ------------------------------------------------------------------ */
+/* Samsung SRW V2, compression 32773 (SURVEY 8(f)4).                     */
+/*   SamsungV2Decompressor::SamsungV2Decompressor / decompress           */
+/*   decompressors/SamsungV2Decompressor.cpp:85-355                      */
+/*   (one MSB32 stream per row, each starting at the next multiple of 16 */
+/*   bytes of the data; blocks of 16 pixels predicted from the left or   */
+/*   from one / two rows up, every pixel clamped to the bit depth).       */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint64_t in_offset;  /* first byte of the strip, its 16-byte header included    */
+  uint32_t in_size;    /* bytes of the strip; < 2^28                              */
+  uint32_t bits;       /* the container's bits per sample (12 or 14)              */
+  int32_t width;       /* the RawImage's dimensions, which must equal the         */
+  int32_t height;      /* header's                                                */
+  uint8_t header[16];  /* the strip's first 16 bytes (the device reads from
+                          in_offset + 16)                                         */
+  uint64_t out_offset; /* byte offset of image row 0; multiple of 4               */
+  uint32_t out_pitch;  /* bytes; multiple of 4, >= 2 * width                      */
+  uint32_t reserved;   /* 0                                                       */
+} rsb200_samsung2_job;
+
+/* Plan creation runs the constructor's checks in its order (SamsungV2Decompressor.cpp:88-142): bits
+ * other than 12 / 14 (RSB200_ERR_RDE "Unexpected bit per pixel"), in_size < 16 (RSB200_ERR_IOE "Out of
+ * bounds access in ByteStream"), then from the header a bit depth other than bits, opt flags > 7,
+ * dimensions the constructor rejects and dimensions other than width x height (RSB200_ERR_RDE with the
+ * reference's messages).  An out_offset or out_pitch that is not a multiple of 4, a pitch below
+ * 2 * width, in_size >= 2^28 or a non-zero reserved field are refused with RSB200_ERR_ARG.
+ * rsb200_plan_results() per job: RSB200_ERR_RDE or RSB200_ERR_IOE with consumed ==
+ * code << 28 | value << 22 | row << 9 | block of the first failure, code one of RSB200_S2_*, value the
+ * number the message prints (the motion, or the difference bits) and block the block of 16 pixels
+ * (0 for a failure in front of the row's first block, width / 16 for the skip behind its last).  The
+ * image is then as the reference leaves it: the rows before the failing one and the blocks of that
+ * row before the failing block written (the whole row for a failure behind it), nothing else. */
+#define RSB200_S2_START_MOTION 1u /* RDE "At start of image and motion isn't 7. File corrupted?" */
+#define RSB200_S2_MOTION_BEGIN 2u /* RDE "Bad motion %d at the beginning of the row"             */
+#define RSB200_S2_MOTION_END 3u   /* RDE "Bad motion %d at the end of the row"                   */
+#define RSB200_S2_UNDERFLOW 4u    /* RDE "Difference bits underflow. File corrupted?"            */
+#define RSB200_S2_TOO_MANY 5u     /* RDE "Too many difference bits (%u). File corrupted?"        */
+#define RSB200_S2_OVERREAD 6u     /* IOE "Buffer overflow read in BitStreamer"                   */
+#define RSB200_S2_SHORT 7u        /* IOE "Bit stream size is smaller than MaxProcessBytes"       */
+#define RSB200_S2_BYTESTREAM 8u   /* IOE "Out of bounds access in ByteStream"                    */
+int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung2_job* jobs, int njobs,
+                                rsb200_plan** plan);
+
+/* ------------------------------------------------------------------ */
 /* Nikon NEF Huffman codec without split (SURVEY 8(f)2).                 */
 /*   NikonDecompressor::decompress  decompressors/NikonDecompressor.cpp:513-560 */
 /*   (plain MSB bit stream, nikon_tree table, per-parity left predictor, */

@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, SamsungV2Job, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -375,6 +375,15 @@ def samsung1_plan(ctx, jobs):
     ja = (SamsungV1Job * len(jobs))(*jobs)
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_samsung1_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def samsung2_plan(ctx, jobs):
+    """Samsung SRW V2 strips (SamsungV2Decompressor::decompress), one job per frame; job.header holds
+    the strip's first 16 bytes."""
+    ja = (SamsungV2Job * len(jobs))(*jobs)
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_samsung2_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

@@ -368,6 +368,22 @@ int rsb200h_samsung_v1(uint16_t* img_data, int w, int h, int cpp, int pitch, con
   });
 }
 
+// cpp: components per pixel of the image (the constructor refuses anything but 1)
+int rsb200h_samsung_v2(uint16_t* img_data, int w, int h, int cpp, int pitch, const uint8_t* data,
+                       uint32_t size, unsigned bits, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, cpp, pitch, true, 1, 1);
+    SamsungV2Decompressor d(img, ByteStream(data, size), bits);
+    try {
+      d.decompress();
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
                                  uint32_t size, rsb200h_err* e) {
   return guarded(e, [&] {

@@ -855,6 +855,86 @@ void SamsungV1Decompressor::decompress() const {
   engineCheck(rc, "rsb200_plan_results");
 }
 
+// ------------------------------------------------------------------ Samsung V2
+// bits [pos, pos + n) of the 16-byte header read as MSB32 (SamsungV2Decompressor.cpp:103-131)
+static uint32_t samsung2HeaderBits(const uint8_t* hd, uint32_t pos, uint32_t n) {
+  uint32_t v = 0;
+  for (uint32_t b = pos; b < pos + n; ++b) {
+    const uint8_t* w = hd + 4 * (b >> 5);
+    const uint32_t word = (uint32_t)w[0] | (uint32_t)w[1] << 8 | (uint32_t)w[2] << 16 | (uint32_t)w[3] << 24;
+    v = v << 1 | ((word >> (31u - (b & 31u))) & 1u);
+  }
+  return v;
+}
+
+SamsungV2Decompressor::SamsungV2Decompressor(const RawImage& image, ByteStream bs_, unsigned bits_)
+    : mRaw(image), bs(bs_), bits(bits_) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||
+      mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  if (bits != 12 && bits != 14)
+    ThrowRDE("Unexpected bit per pixel (%u)", bits);
+  (void)bs.check(16);
+  const uint8_t* hd = bs.begin() + bs.getPosition();
+  const uint32_t depth = samsung2HeaderBits(hd, 20, 4) + 1;
+  if (depth != bits)
+    ThrowRDE("Bit depth mismatch with container, %u vs %u", depth, bits);
+  const uint32_t flags = samsung2HeaderBits(hd, 84, 4);
+  if (flags > 7)
+    ThrowRDE("Invalid opt flags %x", flags);
+  const int width = (int)samsung2HeaderBits(hd, 32, 16), height = (int)samsung2HeaderBits(hd, 48, 16);
+  if (width == 0 || height == 0 || width % 16 != 0 || width > 6496 || height > 4336)
+    ThrowRDE("Unexpected image dimensions found: (%i; %i)", width, height);
+  if (width != mRaw->dim.x || height != mRaw->dim.y)
+    ThrowRDE("EXIF image dimensions do not match dimensions from raw header");
+}
+
+void SamsungV2Decompressor::decompress() const {
+  rsb200_samsung2_job job;
+  std::memset(&job, 0, sizeof job);
+  job.in_offset = 0;
+  // A frame reads at most 283 bits per block (scale 2 + 12, motion 1 + 3, skip 1, flags 8, lengths 16,
+  // differences 16 x 15) and skips at most 15 bytes per row; more data behind that (and the pump's
+  // 8-byte over-read) changes no outcome, so the plan gets no more of it.
+  const uint64_t most = 16 + (uint64_t)mRaw->dim.y * ((283ull * (mRaw->dim.x / 16) + 7) / 8 + 15) + 64;
+  job.in_size = (uint32_t)std::min<uint64_t>(bs.getRemainSize(), most);
+  job.bits = bits;
+  job.width = mRaw->dim.x;
+  job.height = mRaw->dim.y;
+  std::memcpy(job.header, bs.begin() + bs.getPosition(), 16);
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  PlanGuard pg;
+  engineCheck(rsb200_samsung2_plan_create(engine(), &job, 1, &pg.p), "rsb200_samsung2_plan_create");
+  RawImage img = mRaw;
+  runOnImage(pg.p, bs.begin() + bs.getPosition(), job.in_size, img, /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  const unsigned value = (res.consumed >> 22) & 31u;
+  switch (res.consumed >> 28) { // SamsungV2Decompressor.cpp:180-247, 329-350; BitStreamer.h; ByteStream.h
+  case RSB200_S2_START_MOTION:
+    ThrowRDE("At start of image and motion isn't 7. File corrupted?");
+  case RSB200_S2_MOTION_BEGIN:
+    ThrowRDE("Bad motion %d at the beginning of the row", (int)value);
+  case RSB200_S2_MOTION_END:
+    ThrowRDE("Bad motion %d at the end of the row", (int)value);
+  case RSB200_S2_UNDERFLOW:
+    ThrowRDE("Difference bits underflow. File corrupted?");
+  case RSB200_S2_TOO_MANY:
+    ThrowRDE("Too many difference bits (%u). File corrupted?", value);
+  case RSB200_S2_OVERREAD:
+    ThrowIOE("Buffer overflow read in BitStreamer");
+  case RSB200_S2_SHORT:
+    ThrowIOE("Bit stream size is smaller than MaxProcessBytes");
+  case RSB200_S2_BYTESTREAM:
+    ThrowIOE("Out of bounds access in ByteStream");
+  default:
+    engineCheck(rc, "rsb200_plan_results");
+  }
+}
+
 // ------------------------------------------------------------------ Sony ARW1
 SonyArw1Decompressor::SonyArw1Decompressor(RawImage img) : mRaw(std::move(img)) {
   if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||

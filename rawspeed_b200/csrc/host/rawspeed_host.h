@@ -611,6 +611,22 @@ private:
   ByteStream bs;
 };
 
+// ---------------------------------------------------------------- Samsung V2
+// decompressors/SamsungV2Decompressor.h: same constructor (image, stream, bits per sample; its checks,
+// SamsungV2Decompressor.cpp:85-143, in its order, with the 16-byte header read on the host) and
+// decompress().  The rows are decoded on the device (samsung2.cuh); errors are thrown with the
+// reference's classes and messages, printed values included.
+class SamsungV2Decompressor final {
+public:
+  SamsungV2Decompressor(const RawImage& image, ByteStream bs, unsigned bits);
+  void decompress() const;
+
+private:
+  RawImage mRaw;
+  ByteStream bs;
+  unsigned bits;
+};
+
 // ---------------------------------------------------------------- Sony ARW1
 // decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
 // SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs

@@ -31,6 +31,7 @@
 #include "arw1.cuh"
 #include "samsung0.cuh"
 #include "samsung1.cuh"
+#include "samsung2.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -296,6 +297,18 @@ struct rsb200_plan {
   uint32_t* d_s0_jobfail = nullptr;
   uint2* d_s0_res = nullptr;
   uint2* h_s0_res = nullptr; // pinned
+  // Samsung V2 (samsung2.cuh); per-job results go through d_s0_res / h_s0_res as for V0
+  S2FrameDev* d_s2_frames = nullptr;
+  uint32_t* d_s2_starts = nullptr; // per frame, four searches: candidate entries, pair steps, rows, checkpoints
+  uint32_t* d_s2_tab = nullptr;    // candidate entries
+  uint32_t* d_s2_jump = nullptr;   // two ping-pong buffers of s2_njump
+  uint32_t* d_s2_rowstart = nullptr;
+  uint32_t* d_s2_cp = nullptr;
+  uint32_t* d_s2_ncp = nullptr;
+  uint2* d_s2_fail = nullptr;
+  uint2* d_s2_desc = nullptr;
+  int16_t* d_s2_px = nullptr;
+  uint32_t s2_ntab = 0, s2_njump = 0, s2_nrows = 0, s2_ncp = 0;
   uint32_t s0_nrows = 0, s0_nnodes = 0, s0_max_nodes = 0, s0_max_w = 0, s0_max_tiles = 0;
   int s0_rounds = 0;
   // Sony ARW2
@@ -1455,6 +1468,130 @@ static cudaError_t run_samsung0(const rsb200_plan* p, const uint8_t* in, uint8_t
                                                                                      p->d_s0_carry);
   s0_store_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, src, p->d_s0_carry,
                                             p->d_s0_rowfail, p->d_s0_jobfail, outp, p->d_s0_res);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------
+// Samsung V2: one strip per frame, a stream per row at 16-byte boundaries (samsung2.cuh)
+// ------------------------------------------------------------------
+extern "C" int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung2_job* jobs, int njobs,
+                                           rsb200_plan** out) {
+  if (!ctx || !jobs || njobs <= 0 || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "samsung2_plan_create: bad arguments");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung2_job& j = jobs[i];
+    // SamsungV2Decompressor ctor (SamsungV2Decompressor.cpp:88-142), in its order
+    if (j.bits != 12 && j.bits != 14)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected bit per pixel (%u)", i, j.bits);
+    if (j.in_size < 16)
+      return set_err(ctx, RSB200_ERR_IOE, "job %d: Out of bounds access in ByteStream", i);
+    const uint32_t depth = s2_header_bits(j.header, 20, 4) + 1;
+    if (depth != j.bits)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Bit depth mismatch with container, %u vs %u", i, depth, j.bits);
+    const uint32_t flags = s2_header_bits(j.header, 84, 4);
+    if (flags > 7)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Invalid opt flags %x", i, flags);
+    const uint32_t hw = s2_header_bits(j.header, 32, 16), hh = s2_header_bits(j.header, 48, 16);
+    if (hw == 0 || hh == 0 || hw % 16 != 0 || hw > 6496 || hh > 4336)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected image dimensions found: (%i; %i)", i, (int)hw, (int)hh);
+    if ((int32_t)hw != j.width || (int32_t)hh != j.height)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: EXIF image dimensions do not match dimensions from raw header", i);
+    // the reconstruction stores two pixels as one 32-bit word
+    if (j.in_size >= (1u << 28) || (uint64_t)j.width * 2 > j.out_pitch || (j.out_offset % 4) || (j.out_pitch % 4) ||
+        j.reserved)
+      return set_err(ctx, RSB200_ERR_ARG, "samsung2 job %d: malformed descriptor", i);
+  }
+  rsb200_plan* p = new (std::nothrow) rsb200_plan();
+  if (!p)
+    return RSB200_ERR_CUDA;
+  p->ctx = ctx;
+  p->kind = 13;
+  p->nunits = njobs;
+  std::vector<S2FrameDev> fr((size_t)njobs);
+  std::vector<uint32_t> starts((size_t)njobs * 4);
+  S2Totals t;
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_samsung2_job& j = jobs[i];
+    S2FrameDev& f = fr[(size_t)i];
+    s2_place_frame(f, t, starts.data(), (uint32_t)njobs, (uint32_t)i, j.in_offset, j.in_size, j.header, j.bits,
+                   (uint32_t)j.width, (uint32_t)j.height, j.out_offset, j.out_pitch);
+    if (t.tab >= (1ull << 31) || t.rows >= (1ull << 31)) {
+      delete p;
+      return set_err(ctx, RSB200_ERR_ARG, "samsung2 plan: too many frames for one plan");
+    }
+    p->in_bytes += j.in_size;
+    p->out_bytes += (uint64_t)f.w * f.h * 2;
+    p->pixels += (uint64_t)f.w * f.h;
+    p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
+    p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)f.h - 1) * j.out_pitch + 2ull * f.w));
+  }
+  const uint64_t tab = t.tab, jump = t.jump, rows = t.rows, cps = t.cps, desc = t.desc, px = t.px;
+  p->s2_ntab = (uint32_t)tab;
+  p->s2_njump = (uint32_t)jump;
+  p->s2_nrows = (uint32_t)rows;
+  p->s2_ncp = (uint32_t)cps;
+  cudaError_t e = rsb_dev_alloc(&p->d_s2_frames, sizeof(S2FrameDev) * fr.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_s2_frames, fr.data(), sizeof(S2FrameDev) * fr.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_starts, sizeof(uint32_t) * starts.size());
+  if (e == cudaSuccess)
+    e = cudaMemcpy(p->d_s2_starts, starts.data(), sizeof(uint32_t) * starts.size(), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_tab, sizeof(uint32_t) * tab);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_jump, sizeof(uint32_t) * 2 * jump);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_rowstart, sizeof(uint32_t) * rows);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_cp, sizeof(uint32_t) * cps);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_ncp, sizeof(uint32_t) * (size_t)njobs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_fail, sizeof(uint2) * (size_t)njobs);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_desc, sizeof(uint2) * desc);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s2_px, sizeof(int16_t) * px);
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&p->d_s0_res, sizeof(uint2) * (size_t)njobs);
+  if (e == cudaSuccess)
+    e = rsb_host_alloc((void**)&p->h_s0_res, sizeof(uint2) * (size_t)njobs);
+  if (e != cudaSuccess) {
+    rsb200_plan_destroy(p);
+    return set_err(ctx, RSB200_ERR_CUDA, "samsung2 plan allocation failed: %s", cudaGetErrorString(e));
+  }
+  p->launches_per_run = 7 + S2_JUMP;
+  *out = p;
+  return RSB200_OK;
+}
+
+static cudaError_t run_samsung2(const rsb200_plan* p, const uint8_t* in, uint8_t* outp, cudaStream_t st) {
+  const uint32_t nf = (uint32_t)p->nunits;
+  const uint32_t* s = p->d_s2_starts;
+  s2_cand_kernel<<<(p->s2_ntab + S2W_NT - 1) / S2W_NT, S2W_NT, 0, st>>>(in, p->d_s2_frames, s, nf, p->s2_ntab,
+                                                                         p->d_s2_tab);
+  uint32_t* src = p->d_s2_jump;
+  uint32_t* dst = p->d_s2_jump + p->s2_njump;
+  const uint32_t gj = (p->s2_njump + S2J_NT - 1) / S2J_NT;
+  s2_pair_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames, s + nf, nf, p->s2_njump, p->d_s2_tab, src);
+  for (int r = 0; r < S2_JUMP; ++r) {
+    s2_double_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames, s + nf, nf, p->s2_njump, src, dst);
+    std::swap(src, dst);
+  }
+  s2_coarse_kernel<<<(nf + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames, nf, p->d_s2_tab, src,
+                                                                   p->d_s2_rowstart, p->d_s2_cp, p->d_s2_ncp,
+                                                                   p->d_s2_fail);
+  s2_fine_kernel<<<(p->s2_ncp + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames, s + 3 * nf, nf, p->s2_ncp,
+                                                                        p->d_s2_tab, p->d_s2_cp, p->d_s2_ncp,
+                                                                        p->d_s2_rowstart, p->d_s2_fail);
+  s2_desc_kernel<<<(p->s2_nrows + S2W_NT - 1) / S2W_NT, S2W_NT, 0, st>>>(
+      in, p->d_s2_frames, s + 2 * nf, nf, p->s2_nrows, p->d_s2_rowstart, p->d_s2_fail, p->d_s2_desc);
+  s2_diff_kernel<<<p->s2_nrows, S2X_NT, 0, st>>>(in, p->d_s2_frames, s + 2 * nf, nf, p->d_s2_fail, p->d_s2_desc,
+                                                 p->d_s2_px);
+  s2_recon_kernel<<<nf, S2R_NT, 0, st>>>(p->d_s2_frames, p->d_s2_fail, p->d_s2_desc, p->d_s2_px, outp,
+                                         p->d_s0_res);
   return cudaGetLastError();
 }
 
@@ -2839,6 +2976,9 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
   } else if (p->kind == 12) {
     CUDA_TRY(ctx, run_samsung0(p, in, outp, st));
     ctx->launches += (uint64_t)p->launches_per_run;
+  } else if (p->kind == 13) {
+    CUDA_TRY(ctx, run_samsung2(p, in, outp, st));
+    ctx->launches += (uint64_t)p->launches_per_run;
   } else if (p->kind == 5) {
     for (const PanaGroup& g : p->pana_groups) {
       CUDA_TRY(ctx, run_pana_group(p, g, in, outp, st));
@@ -3655,6 +3795,35 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
+  if (p->kind == 13) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_s0_res, p->d_s0_res, sizeof(uint2) * (size_t)p->nunits,
+                                  cudaMemcpyDeviceToHost, p->last_stream));
+    CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
+    // SamsungV2Decompressor.cpp:180-247, 329-350; BitStreamer.h; ByteStream::check
+    static const char* const msgs[9] = {"", "At start of image and motion isn't 7. File corrupted?",
+                                        "Bad motion %u at the beginning of the row",
+                                        "Bad motion %u at the end of the row",
+                                        "Difference bits underflow. File corrupted?",
+                                        "Too many difference bits (%u). File corrupted?",
+                                        "Buffer overflow read in BitStreamer",
+                                        "Bit stream size is smaller than MaxProcessBytes",
+                                        "Out of bounds access in ByteStream"};
+    int first = RSB200_OK;
+    for (int i = 0; i < p->nunits; ++i) {
+      const uint2 r = p->h_s0_res[i];
+      if (results && i < n) {
+        results[i].status = r.x;
+        results[i].consumed = r.y;
+      }
+      if (r.x != RSB200_OK && first == RSB200_OK) {
+        first = (int)r.x;
+        char m[96];
+        snprintf(m, sizeof m, msgs[std::min(r.y >> 28, 8u)], (r.y >> 22) & 31u);
+        set_err(ctx, first, "job %d: %s (row %u, block %u)", i, m, (r.y >> 9) & 0x1FFFu, r.y & 0x1FFu);
+      }
+    }
+    return first;
+  }
   if (p->kind == 11) {
     CUDA_TRY(ctx, cudaMemcpyAsync(p->h_hass_states, p->d_hass_states, sizeof(DevHassState) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
@@ -3834,6 +4003,9 @@ extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
   }
   if (p->kind == 2)
     return p->raw_groups.empty() ? "(empty raw-form plan)" : "rawform_kernel";
+  if (p->kind == 13)
+    return "s2_cand_kernel + s2_pair_kernel + s2_double_kernel + s2_coarse_kernel + s2_fine_kernel + s2_desc_kernel + "
+           "s2_diff_kernel + s2_recon_kernel";
   if (p->kind == 12)
     return "s0_walk_kernel + s0_diff_kernel + s0_node_kernel + s0_jump_kernel + s0_scan_kernel + s0_carry_kernel + "
            "s0_store_kernel";
@@ -3907,6 +4079,16 @@ extern "C" void rsb200_plan_destroy(rsb200_plan* p) {
   rsb_dev_free(p->d_s0_rowfail);
   rsb_dev_free(p->d_s0_jobfail);
   rsb_dev_free(p->d_s0_res);
+  rsb_dev_free(p->d_s2_frames);
+  rsb_dev_free(p->d_s2_starts);
+  rsb_dev_free(p->d_s2_tab);
+  rsb_dev_free(p->d_s2_jump);
+  rsb_dev_free(p->d_s2_rowstart);
+  rsb_dev_free(p->d_s2_cp);
+  rsb_dev_free(p->d_s2_ncp);
+  rsb_dev_free(p->d_s2_fail);
+  rsb_dev_free(p->d_s2_desc);
+  rsb_dev_free(p->d_s2_px);
   if (p->h_s0_res)
     rsb_host_free(p->h_s0_res);
   rsb_dev_free(p->d_p1_strips);

@@ -1,0 +1,39 @@
+"""The Samsung V2 struct of include/rawspeed_b200.h against its ctypes mirror, and the new entry
+points in the export lists."""
+import ctypes as C
+import os
+import subprocess
+
+from rawspeed_b200 import _abi, host
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def test_struct_layout_matches_header(tmp_path):
+    prog = tmp_path / "layout.c"
+    prog.write_text(r'''
+#include <stdio.h>
+#include <stddef.h>
+#include "rawspeed_b200.h"
+int main(void){
+  printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", sizeof(rsb200_samsung2_job),
+         offsetof(rsb200_samsung2_job, in_offset), offsetof(rsb200_samsung2_job, in_size),
+         offsetof(rsb200_samsung2_job, bits), offsetof(rsb200_samsung2_job, width),
+         offsetof(rsb200_samsung2_job, height), offsetof(rsb200_samsung2_job, header),
+         offsetof(rsb200_samsung2_job, out_offset),
+         offsetof(rsb200_samsung2_job, out_pitch), offsetof(rsb200_samsung2_job, reserved));
+  return 0;
+}
+''')
+    exe = tmp_path / "layout"
+    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(prog)])
+    got = [int(x) for x in subprocess.check_output([str(exe)], text=True).split()]
+    J = _abi.SamsungV2Job
+    want = [C.sizeof(J), J.in_offset.offset, J.in_size.offset, J.bits.offset, J.width.offset,
+            J.height.offset, J.header.offset, J.out_offset.offset, J.out_pitch.offset, J.reserved.offset]
+    assert got == want
+
+
+def test_entry_points_listed():
+    assert "rsb200_samsung2_plan_create" in _abi.EXPORTS
+    assert "rsb200h_samsung_v2" in host.EXPORTS
