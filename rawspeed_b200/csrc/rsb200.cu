@@ -66,9 +66,6 @@ static cudaError_t rsb_dev_alloc(void** p, size_t n) {
   }
   return e;
 }
-template <typename T> static cudaError_t rsb_dev_alloc(T** p, size_t n) {
-  return rsb_dev_alloc(reinterpret_cast<void**>(p), n);
-}
 static cudaError_t rsb_dev_free(void* p) {
   if (!p)
     return cudaSuccess;
@@ -112,9 +109,6 @@ static cudaError_t rsb_host_alloc(void** p, size_t n) {
   }
   return e;
 }
-template <typename T> static cudaError_t rsb_host_alloc(T** p, size_t n) {
-  return rsb_host_alloc(reinterpret_cast<void**>(p), n);
-}
 static cudaError_t rsb_host_free(void* p) {
   if (!p)
     return cudaSuccess;
@@ -126,6 +120,41 @@ static cudaError_t rsb_host_free(void* p) {
   c.free_blocks.emplace(it->second, p);
   c.live.erase(it);
   return cudaSuccess;
+}
+
+// Owners of a plan's device memory and of its pinned result buffers (read on the host by index);
+// null means "not allocated".
+struct DevFree {
+  void operator()(void* p) const { rsb_dev_free(p); }
+};
+struct HostFree {
+  void operator()(void* p) const { rsb_host_free(p); }
+};
+template <class T> using DevPtr = std::unique_ptr<T, DevFree>;
+template <class T> using PinnedPtr = std::unique_ptr<T[], HostFree>;
+
+// A create chains its allocations through `e`: each step does nothing once an earlier one failed,
+// so the create checks `e` once.  An empty request still gets 16 bytes (kernels are never handed null).
+template <class T> static void dev_alloc(cudaError_t& e, DevPtr<T>& d, size_t bytes) {
+  void* raw = nullptr;
+  if (e == cudaSuccess)
+    e = rsb_dev_alloc(&raw, bytes ? bytes : 16);
+  if (e == cudaSuccess)
+    d.reset(static_cast<T*>(raw));
+}
+// ... and copies `bytes` from the host into it; `pad` more bytes behind them are allocated, not copied
+template <class T>
+static void dev_upload(cudaError_t& e, DevPtr<T>& d, const void* src, size_t bytes, size_t pad = 0) {
+  dev_alloc(e, d, bytes + pad);
+  if (e == cudaSuccess && bytes)
+    e = cudaMemcpy(d.get(), src, bytes, cudaMemcpyHostToDevice);
+}
+template <class T> static void host_alloc(cudaError_t& e, PinnedPtr<T>& h, size_t bytes) {
+  void* raw = nullptr;
+  if (e == cudaSuccess)
+    e = rsb_host_alloc(&raw, bytes);
+  if (e == cudaSuccess)
+    h.reset(static_cast<T*>(raw));
 }
 
 // ------------------------------------------------------------------
@@ -179,21 +208,21 @@ static inline uint64_t sat_add(uint64_t a, uint64_t b) { return a + b < a ? ~0ul
 struct UnpackGroup {
   int bps_t;  // template bps (0 = generic)
   bool lsb;
-  UnpackJobDev* d_jobs = nullptr;
+  DevPtr<UnpackJobDev> d_jobs;
   int njobs = 0;
   uint32_t nblocks = 0;
 };
 
 struct RawGroup {
   int format = 0;
-  RawJobDev* d_jobs = nullptr;
+  DevPtr<RawJobDev> d_jobs;
   int njobs = 0;
   uint32_t total_items = 0;
 };
 
 struct PanaGroup {
   int version = 0, bps = 0;
-  PanaJobDev* d_jobs = nullptr;
+  DevPtr<PanaJobDev> d_jobs;
   int njobs = 0;
   uint32_t total_units = 0;
 };
@@ -201,14 +230,14 @@ struct PanaGroup {
 struct SrawGroup {
   int version = 0;
   bool is420 = false;
-  SrawJobDev* d_jobs = nullptr;
+  DevPtr<SrawJobDev> d_jobs;
   int njobs = 0;
   uint32_t total_mcus = 0;
 };
 
 struct ScaleGroup {
   int mode = 0; // 0: SSE2 loop semantics, 1: plain loop semantics
-  ScaleJobDev* d_jobs = nullptr;
+  DevPtr<ScaleJobDev> d_jobs;
   int njobs = 0;
   uint32_t total_quads = 0;
   uint32_t nseg = 1; // column segments per row quad (mode 1)
@@ -217,15 +246,36 @@ struct ScaleGroup {
 struct UnpackFastGroup {
   int bps;
   bool lsb;
-  UnpackFastJobDev* d_jobs = nullptr;
+  DevPtr<UnpackFastJobDev> d_jobs;
   int njobs = 0;
   uint32_t nblocks = 0;
   std::vector<UnpackFastJobDev> h_jobs; // host copy (pipelined host runs)
 };
 
+enum class PlanKind {
+  Unpack,
+  Ljpeg, // every LJPEG-family create: ljpeg, cr2, pentax, nikon, arw1, samsung1
+  RawForm,
+  Sraw,
+  Arw2,
+  Pana,
+  PhaseOne,
+  Scale,
+  DngOp,
+  BadPix,
+  Lookup,
+  Hasselblad,
+  SamsungV0,
+  SamsungV2
+};
+
+static bool in_place(PlanKind k) {
+  return k == PlanKind::Scale || k == PlanKind::DngOp || k == PlanKind::BadPix || k == PlanKind::Lookup;
+}
+
 struct rsb200_plan {
   rsb200_ctx* ctx = nullptr;
-  int kind = 0; // 0 unpack, 1 ljpeg/cr2, 2 fixed-layout raw forms, 3 sRaw interpolation, 4 ARW2, 5 Panasonic, 6 Phase One, 7 black/white scaling (in place), 8 DNG opcode list (in place), 9 bad-pixel interpolation (in place), 10 whole-image table lookup (in place), 11 Hasselblad, 12 Samsung V0
+  PlanKind kind = PlanKind::Unpack;
   int nunits = 0;
   uint64_t in_bytes = 0, out_bytes = 0, pixels = 0;
   int launches_per_run = 0;
@@ -236,26 +286,26 @@ struct rsb200_plan {
   std::vector<UnpackFastGroup> fast_groups;
   // fixed-layout raw forms
   std::vector<RawGroup> raw_groups;
-  uint16_t* d_raw_tables = nullptr;
+  DevPtr<uint16_t> d_raw_tables;
   std::vector<SrawGroup> sraw_groups;
   std::vector<PanaGroup> pana_groups;
-  // Panasonic V4 bad-pixel lists: slot per job that asked for them (-1 otherwise)
-  std::vector<int> pana_zero_slot;
-  uint32_t* d_pana_zero_count = nullptr;
-  uint32_t* d_pana_zero_list = nullptr;
-  int pana_zero_slots = 0;
+  // bad-pixel lists of Panasonic V4 jobs and of DNG BAD_CONSTANT opcodes: slot per job / opcode
+  // that asked for one (-1 otherwise)
+  std::vector<int> bad_slot;
+  DevPtr<uint32_t> d_bad_count;
+  DevPtr<uint32_t> d_bad_list;
+  int nbad_slots = 0;
   std::vector<ScaleGroup> scale_groups;
-  // DNG opcode pass (K10); bad-pixel lists share pana_zero_slot / d_pana_zero_* (slot per
-  // BAD_CONSTANT opcode, indexed by opcode)
-  DngOpJobDev* d_dngop_jobs = nullptr;
-  DngOpDev* d_dngop_ops = nullptr;
-  uint16_t* d_dngop_tables = nullptr;
-  uint32_t* d_dngop_deltas = nullptr;
+  // DNG opcode pass (K10)
+  DevPtr<DngOpJobDev> d_dngop_jobs;
+  DevPtr<DngOpDev> d_dngop_ops;
+  DevPtr<uint16_t> d_dngop_tables;
+  DevPtr<uint32_t> d_dngop_deltas;
   int dngop_njobs = 0;
   uint32_t dngop_units = 0;
   // whole-image table lookup (K12)
-  LookupJobDev* d_lookup_jobs = nullptr;
-  uint16_t* d_lookup_tables = nullptr;
+  DevPtr<LookupJobDev> d_lookup_jobs;
+  DevPtr<uint16_t> d_lookup_tables;
   int lookup_njobs = 0;
   uint32_t lookup_quads = 0;
   uint32_t lookup_nseg = 1; // column segments per row quad (more warps for few rows)
@@ -263,78 +313,80 @@ struct rsb200_plan {
   bool lookup_smem = false; // RSB200_LUT_SMEM=1 at plan creation: the shared-memory-table kernel (A/B candidate, lookup.cuh)
   int lookup_ntables = 0;
   // bad-pixel interpolation (K11)
-  BadPixJobDev* d_badpix_jobs = nullptr;
-  uint32_t* d_badpix_list = nullptr;
-  uint8_t* d_badpix_maps = nullptr;
+  DevPtr<BadPixJobDev> d_badpix_jobs;
+  DevPtr<uint32_t> d_badpix_list;
+  DevPtr<uint8_t> d_badpix_maps;
   int badpix_njobs = 0;
   uint32_t badpix_total = 0;
-  // Phase One (shares d_arw2_bad / h_arw2_bad as the per-job error flags)
+  // per-job error flags of ARW2 and Phase One
+  DevPtr<uint32_t> d_job_bad;
+  PinnedPtr<uint32_t> h_job_bad;
+  // per-job results of Samsung V0 and V2
+  DevPtr<uint2> d_job_res;
+  PinnedPtr<uint2> h_job_res;
   // Hasselblad (K2H)
-  DevHassJob* d_hass_jobs = nullptr;
-  DevHassCta* d_hass_ctas = nullptr;
-  DevHassState* d_hass_states = nullptr;
-  DevHassState* h_hass_states = nullptr; // pinned
-  uint32_t* d_hass_seg_job = nullptr;
-  uint32_t* d_hass_u32 = nullptr;        // start | parsed | exit | count (nseg each) | cta_sum | cta_base | changed
-  uint32_t* d_hass_row_begin = nullptr;
+  DevPtr<DevHassJob> d_hass_jobs;
+  DevPtr<DevHassCta> d_hass_ctas;
+  DevPtr<DevHassState> d_hass_states;
+  PinnedPtr<DevHassState> h_hass_states;
+  DevPtr<uint32_t> d_hass_seg_job;
+  DevPtr<uint32_t> d_hass_u32; // start | parsed | exit | count (nseg each) | cta_sum | cta_base | changed
+  DevPtr<uint32_t> d_hass_row_begin;
   uint32_t hass_nseg = 0, hass_ncta = 0, hass_rows = 0;
-  P1StripDev* d_p1_strips = nullptr;
-  P1JobDev* d_p1_jobs = nullptr;
-  uint32_t* d_p1_gdesc = nullptr;   // third version: one word per group of 8 pixels (+ 1 per row)
-  uint32_t* d_p1_rowflag = nullptr; // ... and per row: failed before anything was stored
+  // Phase One (K8)
+  DevPtr<P1StripDev> d_p1_strips;
+  DevPtr<P1JobDev> d_p1_jobs;
+  DevPtr<uint32_t> d_p1_gdesc;   // third version: one word per group of 8 pixels (+ 1 per row)
+  DevPtr<uint32_t> d_p1_rowflag; // ... and per row: failed before anything was stored
   uint32_t p1_gstride = 0;          // words of gdesc per row
   int p1_ver = 3;                   // which version of the kernel this plan runs (RSB200_P1)
   int p1_walk1 = 0;                 // RSB200_P1W = 1 .. 6: other forms of the third version's walk (A/B; see p1_walk_kernel)
   uint32_t p1_nstrips = 0;
   // Samsung V0 (K13, samsung0.cuh)
-  S0RowDev* d_s0_rows = nullptr;
-  S0JobDev* d_s0_jobs = nullptr;
-  uint2* d_s0_desc = nullptr;     // per block
-  uint16_t* d_s0_adj = nullptr;   // per pixel (rows of 16 * blocks)
-  uint2* d_s0_nodes = nullptr;    // two ping-pong buffers of s0_nnodes
-  uint32_t* d_s0_carry = nullptr; // per row tile, column and chain
-  uint32_t* d_s0_rowfail = nullptr;
-  uint32_t* d_s0_jobfail = nullptr;
-  uint2* d_s0_res = nullptr;
-  uint2* h_s0_res = nullptr; // pinned
-  // Samsung V2 (samsung2.cuh); per-job results go through d_s0_res / h_s0_res as for V0
-  S2FrameDev* d_s2_frames = nullptr;
-  uint32_t* d_s2_starts = nullptr; // per frame, four searches: candidate entries, pair steps, rows, checkpoints
-  uint32_t* d_s2_tab = nullptr;    // candidate entries
-  uint32_t* d_s2_jump = nullptr;   // two ping-pong buffers of s2_njump
-  uint32_t* d_s2_rowstart = nullptr;
-  uint32_t* d_s2_cp = nullptr;
-  uint32_t* d_s2_ncp = nullptr;
-  uint2* d_s2_fail = nullptr;
-  uint2* d_s2_desc = nullptr;
-  int16_t* d_s2_px = nullptr;
+  DevPtr<S0RowDev> d_s0_rows;
+  DevPtr<S0JobDev> d_s0_jobs;
+  DevPtr<uint2> d_s0_desc;     // per block
+  DevPtr<uint16_t> d_s0_adj;   // per pixel (rows of 16 * blocks)
+  DevPtr<uint2> d_s0_nodes;    // two ping-pong buffers of s0_nnodes
+  DevPtr<uint32_t> d_s0_carry; // per row tile, column and chain
+  DevPtr<uint32_t> d_s0_rowfail;
+  DevPtr<uint32_t> d_s0_jobfail;
+  // Samsung V2 (samsung2.cuh)
+  DevPtr<S2FrameDev> d_s2_frames;
+  DevPtr<uint32_t> d_s2_starts; // per frame, four searches: candidate entries, pair steps, rows, checkpoints
+  DevPtr<uint32_t> d_s2_tab;    // candidate entries
+  DevPtr<uint32_t> d_s2_jump;   // two ping-pong buffers of s2_njump
+  DevPtr<uint32_t> d_s2_rowstart;
+  DevPtr<uint32_t> d_s2_cp;
+  DevPtr<uint32_t> d_s2_ncp;
+  DevPtr<uint2> d_s2_fail;
+  DevPtr<uint2> d_s2_desc;
+  DevPtr<int16_t> d_s2_px;
   uint32_t s2_ntab = 0, s2_njump = 0, s2_nrows = 0, s2_ncp = 0;
   uint32_t s0_nrows = 0, s0_nnodes = 0, s0_max_nodes = 0, s0_max_w = 0, s0_max_tiles = 0;
   int s0_rounds = 0;
   // Sony ARW2
-  Arw2JobDev* d_arw2_jobs = nullptr;
-  uint16_t* d_arw2_tables = nullptr;
-  uint32_t* d_arw2_bad = nullptr;
-  uint32_t* h_arw2_bad = nullptr; // pinned
+  DevPtr<Arw2JobDev> d_arw2_jobs;
+  DevPtr<uint16_t> d_arw2_tables;
   uint32_t arw2_groups = 0;
   int arw2_mode = 0, arw2_ntables = 0;
   // ljpeg
-  DevTable* d_tables = nullptr;
-  DevScan* d_scans = nullptr;
-  DevStrip* d_strips = nullptr;
-  K3RowRef* d_rows = nullptr;
-  uint16_t* d_diffs = nullptr;
-  uint16_t* d_colvals = nullptr;
-  DevResult* d_results = nullptr;
-  DevResult* h_results = nullptr; // pinned
+  DevPtr<DevTable> d_tables;
+  DevPtr<DevScan> d_scans;
+  DevPtr<DevStrip> d_strips;
+  DevPtr<K3RowRef> d_rows;
+  DevPtr<uint16_t> d_diffs;
+  DevPtr<uint16_t> d_colvals;
+  DevPtr<DevResult> d_results;
+  PinnedPtr<DevResult> h_results;
   uint32_t nrows = 0;
   int nscans = 0;
   int ntab_slots = 4;
   // small LJPEG tile segments: one fused CTA each; big segments (CR2 frames,
   // untiled strips): multi-CTA count/verify/diffs + K3
-  uint32_t* d_small_ids = nullptr;
+  DevPtr<uint32_t> d_small_ids;
   int nsmall = 0;
-  uint32_t* d_tile_ids = nullptr; // segments decoded by k2_tile_kernel<R> (ljpeg_tile.cuh)
+  DevPtr<uint32_t> d_tile_ids; // segments decoded by k2_tile_kernel<R> (ljpeg_tile.cuh)
   // host-buffer runs of a plan that holds only such segments are pipelined group by group
   // (upload / decode / download of consecutive groups overlap on three streams)
   struct TileGroup {
@@ -342,7 +394,7 @@ struct rsb200_plan {
     uint64_t in_lo, in_hi, out_lo, out_hi;
   };
   std::vector<TileGroup> tile_groups;
-  DevTileParam* d_tile_params = nullptr;
+  DevPtr<DevTileParam> d_tile_params;
   int ntile = 0;
   int tile_r = 1;
   bool clean2 = false; // thread path: k2_clean2_kernel instead of k2_clean_kernel
@@ -352,54 +404,66 @@ struct rsb200_plan {
   int stream_form = 0;     // k2_stream_kernel: 0 = by launch size, 1 = prefetch form, 2 = full-launch form (RSB200_STREAM_FORM)
   bool host_tiles_only = false; // tile_groups / d_tile_ids describe the thread path's segments for host-buffer runs only
   std::vector<uint32_t> h_in_size; // per scan: bytes of a plain LJPEG segment (kind 0), else 0xFFFFFFFF
-  DevTileParam* d_thread_tile_params = nullptr; // thread path: parameters of the exact second opinion
-  uint32_t* d_redo = nullptr;                   // ... and which segments need it (written by K2T)
+  DevPtr<DevTileParam> d_thread_tile_params; // thread path: parameters of the exact second opinion
+  DevPtr<uint32_t> d_redo;                   // ... and which segments need it (written by K2T)
   int nthread_redo = 0;                         // segments of the thread path the tile kernel can take
-  uint32_t* d_thread_ids = nullptr; // segments decoded one per thread (K2C + K2T)
-  DevTScan* d_tscans = nullptr;
-  DevTInfo* d_tinfos = nullptr;
-  uint32_t* d_clean = nullptr;      // unstuffed data of those segments
-  uint32_t* d_anchors = nullptr;
+  DevPtr<uint32_t> d_thread_ids; // segments decoded one per thread (K2C + K2T)
+  DevPtr<DevTScan> d_tscans;
+  DevPtr<DevTInfo> d_tinfos;
+  DevPtr<uint32_t> d_clean;      // unstuffed data of those segments
+  DevPtr<uint32_t> d_anchors;
   int nthread = 0;
   int ntables = 0;
-  uint32_t* d_big_ids = nullptr;
+  DevPtr<uint32_t> d_big_ids;
   std::vector<uint32_t> h_big_ids; // (for rsb200_debug_range_redo)
   int nbig = 0;
-  BigScanInfo* d_big = nullptr;
-  DevRange* d_ranges = nullptr;
-  RangeState* d_states = nullptr;
-  RangeFinal* d_finals = nullptr;
-  uint32_t* d_fallback = nullptr;
+  DevPtr<BigScanInfo> d_big;
+  DevPtr<DevRange> d_ranges;
+  DevPtr<RangeState> d_states;
+  DevPtr<RangeFinal> d_finals;
+  DevPtr<uint32_t> d_fallback;
   int nranges = 0;
   // Pentax segments (DevScan::kind == 2): first out-of-bounds pixel per segment
-  uint32_t* d_oob = nullptr;
-  uint32_t* h_oob = nullptr; // pinned
+  DevPtr<uint32_t> d_oob;
+  PinnedPtr<uint32_t> h_oob;
   bool has_pentax = false, has_k3 = false, has_nikon = false;
-  uint16_t* d_nikon_luts = nullptr;
+  DevPtr<uint16_t> d_nikon_luts;
   // Sony ARW1 frames (DevScan::kind == 4, arw1.cuh): the range decoder reads their complemented
   // streams from d_arw1_in
   bool has_arw1 = false;
   int narw1 = 0;
-  DevArw1* d_arw1 = nullptr;
-  uint8_t* d_arw1_in = nullptr;
+  DevPtr<DevArw1> d_arw1;
+  DevPtr<uint8_t> d_arw1_in;
   uint64_t arw1_in_bytes = 0;
-  Arw1Run* d_arw1_runs = nullptr;
-  uint32_t* d_arw1_lastoff = nullptr;
-  int2* d_arw1_runpre = nullptr;
-  Arw1Info* d_arw1_info = nullptr;
+  DevPtr<Arw1Run> d_arw1_runs;
+  DevPtr<uint32_t> d_arw1_lastoff;
+  DevPtr<int2> d_arw1_runpre;
+  DevPtr<Arw1Info> d_arw1_info;
   uint32_t arw1_max_runs = 0, arw1_max_tiles = 0, arw1_max_words = 0;
   // Samsung V1 frames (DevScan::kind == 5, samsung1.cuh): reconstruction and end-of-stream scratch
   bool has_samsung1 = false;
   int ns1 = 0;
-  DevS1* d_s1 = nullptr;
-  uint16_t* d_s1_colvals = nullptr; // 2 per row
-  uint2* d_s1_rowbits = nullptr;    // per row
-  uint32_t* d_s1_oob = nullptr;     // per frame: first out-of-range pixel
-  uint32_t* d_s1_lim = nullptr;     // per frame: first pixel not written
+  DevPtr<DevS1> d_s1;
+  DevPtr<uint16_t> d_s1_colvals; // 2 per row
+  DevPtr<uint2> d_s1_rowbits;    // per row
+  DevPtr<uint32_t> d_s1_oob;     // per frame: first out-of-range pixel
+  DevPtr<uint32_t> d_s1_lim;     // per frame: first pixel not written
   uint32_t s1_max_h = 0;
   cudaStream_t last_stream = nullptr;
   bool ran = false;
 };
+
+// A create builds its plan in a holder, so that every refusal frees whatever it allocated so far,
+// and hands it out with `*out = holder.release()`.  Null when out of memory.
+using PlanHolder = std::unique_ptr<rsb200_plan, decltype(&rsb200_plan_destroy)>;
+static PlanHolder new_plan(rsb200_ctx* ctx, PlanKind kind) {
+  PlanHolder holder(new (std::nothrow) rsb200_plan(), rsb200_plan_destroy);
+  if (holder) {
+    holder->ctx = ctx;
+    holder->kind = kind;
+  }
+  return holder;
+}
 
 extern "C" int rsb200_abi_version(void) { return RSB200_ABI_VERSION; }
 
@@ -540,11 +604,10 @@ extern "C" int rsb200_unpack_plan_create(rsb200_ctx* ctx, const rsb200_unpack_jo
   if (!ctx || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "unpack_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Unpack);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 0;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::map<std::pair<int, bool>, std::vector<UnpackJobDev>> buckets;
   std::map<std::pair<int, bool>, std::vector<UnpackFastJobDev>> fast_buckets;
@@ -556,10 +619,8 @@ extern "C" int rsb200_unpack_plan_create(rsb200_ctx* ctx, const rsb200_unpack_jo
         ((uint64_t)j.samples * (uint64_t)j.bps) % 8 != 0 ||
         (uint64_t)j.in_pitch < ((uint64_t)j.samples * j.bps) / 8 ||
         (uint64_t)j.rows * (uint64_t)j.in_pitch > j.in_size ||
-        ((uint64_t)j.out_col0 + j.samples) * 2 > (uint64_t)j.out_pitch) {
-      delete p;
+        ((uint64_t)j.out_col0 + j.samples) * 2 > (uint64_t)j.out_pitch)
       return set_err(ctx, RSB200_ERR_ARG, "unpack job %d: malformed descriptor", i);
-    }
     if (j.rows == 0)
       continue;
     UnpackJobDev d;
@@ -624,16 +685,12 @@ extern "C" int rsb200_unpack_plan_create(rsb200_ctx* ctx, const rsb200_unpack_jo
     }
     g.njobs = (int)kv.second.size();
     g.nblocks = nb;
-    cudaError_t e = rsb_dev_alloc(&g.d_jobs, sizeof(UnpackJobDev) * kv.second.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(g.d_jobs, kv.second.data(), sizeof(UnpackJobDev) * kv.second.size(),
-                     cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, kv.second.data(), sizeof(UnpackJobDev) * kv.second.size());
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "unpack plan upload failed: %s",
                      cudaGetErrorString(e));
-    }
-    p->groups.push_back(g);
+    p->groups.push_back(std::move(g));
   }
   for (auto& kv : fast_buckets) {
     UnpackFastGroup g;
@@ -647,19 +704,15 @@ extern "C" int rsb200_unpack_plan_create(rsb200_ctx* ctx, const rsb200_unpack_jo
     g.njobs = (int)kv.second.size();
     g.nblocks = nb;
     g.h_jobs = kv.second;
-    cudaError_t e = rsb_dev_alloc(&g.d_jobs, sizeof(UnpackFastJobDev) * kv.second.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(g.d_jobs, kv.second.data(), sizeof(UnpackFastJobDev) * kv.second.size(),
-                     cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, kv.second.data(), sizeof(UnpackFastJobDev) * kv.second.size());
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "unpack plan upload failed: %s",
                      cudaGetErrorString(e));
-    }
-    p->fast_groups.push_back(g);
+    p->fast_groups.push_back(std::move(g));
   }
   p->launches_per_run = (int)(p->groups.size() + p->fast_groups.size());
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -671,11 +724,10 @@ extern "C" int rsb200_raw_plan_create(rsb200_ctx* ctx, const rsb200_raw_job* job
   if (!ctx || !jobs || njobs <= 0 || !out || ntables < 0 || (ntables > 0 && !tables))
     return set_err(ctx, RSB200_ERR_ARG, "raw_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::RawForm);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 2;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::map<int, std::vector<RawJobDev>> buckets;
   for (int i = 0; i < njobs; ++i) {
@@ -698,10 +750,8 @@ extern "C" int rsb200_raw_plan_create(rsb200_ctx* ctx, const rsb200_raw_job* job
       if (j.format == RSB200_RAW_8BIT_TABLE)
         ok = ok && j.table >= 0 && j.table < ntables;
     }
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "raw job %d: malformed descriptor", i);
-    }
     if (j.rows == 0)
       continue;
     RawJobDev d;
@@ -718,10 +768,8 @@ extern "C" int rsb200_raw_plan_create(rsb200_ctx* ctx, const rsb200_raw_job* job
     d.table = (uint32_t)j.table;
     const uint32_t K = raw_item_samples(j.format);
     d.ipr = ((uint32_t)j.samples + K - 1) / K;
-    if ((uint64_t)d.ipr * d.rows >= 0xFFFF0000ull) {
-      delete p;
+    if ((uint64_t)d.ipr * d.rows >= 0xFFFF0000ull)
       return set_err(ctx, RSB200_ERR_ARG, "raw job %d: too large", i);
-    }
     buckets[j.format].push_back(d);
     p->in_bytes += (uint64_t)j.rows * raw_in_bytes(j.format, (uint32_t)j.samples);
     p->out_bytes += (uint64_t)j.rows * (uint64_t)j.samples * ob;
@@ -731,14 +779,10 @@ extern "C" int rsb200_raw_plan_create(rsb200_ctx* ctx, const rsb200_raw_job* job
                          (uint64_t)ob * ((uint64_t)j.out_col0 + j.samples)));
   }
   if (ntables > 0) {
-    const size_t tb = (size_t)ntables * 65536u * sizeof(uint16_t);
-    cudaError_t e = rsb_dev_alloc(&p->d_raw_tables, tb);
-    if (e == cudaSuccess)
-      e = cudaMemcpy(p->d_raw_tables, tables, tb, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, p->d_raw_tables, tables, (size_t)ntables * 65536u * sizeof(uint16_t));
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "raw plan upload failed: %s", cudaGetErrorString(e));
-    }
   }
   for (auto& kv : buckets) {
     RawGroup g;
@@ -748,24 +792,18 @@ extern "C" int rsb200_raw_plan_create(rsb200_ctx* ctx, const rsb200_raw_job* job
       d.item_begin = (uint32_t)items;
       items += (uint64_t)d.ipr * d.rows;
     }
-    if (items >= 0xFFFF0000ull) {
-      rsb200_plan_destroy(p);
+    if (items >= 0xFFFF0000ull)
       return set_err(ctx, RSB200_ERR_ARG, "raw plan: too many items of format %d", g.format);
-    }
     g.total_items = (uint32_t)items;
     g.njobs = (int)kv.second.size();
-    cudaError_t e = rsb_dev_alloc(&g.d_jobs, sizeof(RawJobDev) * kv.second.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(g.d_jobs, kv.second.data(), sizeof(RawJobDev) * kv.second.size(),
-                     cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, kv.second.data(), sizeof(RawJobDev) * kv.second.size());
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "raw plan upload failed: %s", cudaGetErrorString(e));
-    }
-    p->raw_groups.push_back(g);
+    p->raw_groups.push_back(std::move(g));
   }
   p->launches_per_run = (int)p->raw_groups.size();
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -773,7 +811,7 @@ template <int FORMAT>
 static cudaError_t launch_rawform(const RawGroup& g, const uint8_t* in, uint64_t in_total,
                                   uint8_t* outp, const uint16_t* tables, cudaStream_t st) {
   const uint32_t nb = (g.total_items + RAW_NT - 1) / RAW_NT;
-  rawform_kernel<FORMAT><<<nb, RAW_NT, 0, st>>>(in, in_total, outp, g.d_jobs, g.njobs,
+  rawform_kernel<FORMAT><<<nb, RAW_NT, 0, st>>>(in, in_total, outp, g.d_jobs.get(), g.njobs,
                                                 g.total_items, tables);
   return cudaGetLastError();
 }
@@ -811,10 +849,10 @@ extern "C" int rsb200_lookup_plan_create(rsb200_ctx* ctx, const rsb200_lookup_jo
   if (!ctx || !jobs || njobs <= 0 || !out || !tables || ntables <= 0)
     return set_err(ctx, RSB200_ERR_ARG, "lookup_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  std::unique_ptr<rsb200_plan, void (*)(rsb200_plan*)> holder(new rsb200_plan, rsb200_plan_destroy);
+  PlanHolder holder = new_plan(ctx, PlanKind::Lookup);
+  if (!holder)
+    return RSB200_ERR_CUDA;
   rsb200_plan* p = holder.get();
-  p->ctx = ctx;
-  p->kind = 10;
   p->nunits = njobs;
   p->lookup_dither = dither != 0;
   {
@@ -848,12 +886,11 @@ extern "C" int rsb200_lookup_plan_create(rsb200_ctx* ctx, const rsb200_lookup_jo
     if (const char* e = getenv("RSB200_LUT_NSEG"))
       p->lookup_nseg = (uint32_t)std::max(1, std::min(64, atoi(e)));
   }
-  const size_t tbytes = sizeof(uint16_t) * (size_t)ntables * (dither ? 131072u : 65536u);
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_lookup_jobs, sizeof(LookupJobDev) * hj.size()));
-  CUDA_TRY(ctx, cudaMemcpy(p->d_lookup_jobs, hj.data(), sizeof(LookupJobDev) * hj.size(),
-                           cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_lookup_tables, tbytes));
-  CUDA_TRY(ctx, cudaMemcpy(p->d_lookup_tables, tables, tbytes, cudaMemcpyHostToDevice));
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_lookup_jobs, hj.data(), sizeof(LookupJobDev) * hj.size());
+  dev_upload(e, p->d_lookup_tables, tables, sizeof(uint16_t) * (size_t)ntables * (dither ? 131072u : 65536u));
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "lookup plan upload failed: %s", cudaGetErrorString(e));
   p->launches_per_run = 1;
   *out = holder.release();
   return RSB200_OK;
@@ -866,10 +903,10 @@ extern "C" int rsb200_badpix_plan_create(rsb200_ctx* ctx, const rsb200_badpix_jo
   if (!ctx || !jobs || njobs <= 0 || !out || (npositions && !positions))
     return set_err(ctx, RSB200_ERR_ARG, "badpix_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  std::unique_ptr<rsb200_plan, void (*)(rsb200_plan*)> holder(new rsb200_plan, rsb200_plan_destroy);
+  PlanHolder holder = new_plan(ctx, PlanKind::BadPix);
+  if (!holder)
+    return RSB200_ERR_CUDA;
   rsb200_plan* p = holder.get();
-  p->ctx = ctx;
-  p->kind = 9;
   p->nunits = njobs;
   std::vector<BadPixJobDev> hj((size_t)njobs);
   std::vector<uint8_t> maps;
@@ -887,16 +924,12 @@ extern "C" int rsb200_badpix_plan_create(rsb200_ctx* ctx, const rsb200_badpix_jo
     return set_err(ctx, RSB200_ERR_ARG, "badpix plan: too many bad pixels");
   p->badpix_njobs = njobs;
   p->badpix_total = (uint32_t)list.size();
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_badpix_jobs, sizeof(BadPixJobDev) * hj.size()));
-  CUDA_TRY(ctx, cudaMemcpy(p->d_badpix_jobs, hj.data(), sizeof(BadPixJobDev) * hj.size(),
-                           cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_badpix_list, sizeof(uint32_t) * (list.size() + 1)));
-  if (!list.empty())
-    CUDA_TRY(ctx, cudaMemcpy(p->d_badpix_list, list.data(), sizeof(uint32_t) * list.size(),
-                             cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_badpix_maps, maps.size() + 16));
-  if (!maps.empty())
-    CUDA_TRY(ctx, cudaMemcpy(p->d_badpix_maps, maps.data(), maps.size(), cudaMemcpyHostToDevice));
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_badpix_jobs, hj.data(), sizeof(BadPixJobDev) * hj.size());
+  dev_upload(e, p->d_badpix_list, list.data(), sizeof(uint32_t) * list.size(), sizeof(uint32_t));
+  dev_upload(e, p->d_badpix_maps, maps.data(), maps.size(), 16);
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "badpix plan upload failed: %s", cudaGetErrorString(e));
   p->launches_per_run = p->badpix_total ? 1 : 0;
   *out = holder.release();
   return RSB200_OK;
@@ -912,17 +945,17 @@ extern "C" int rsb200_dngop_plan_create(rsb200_ctx* ctx, const rsb200_dngop_job*
       (ntables > 0 && !tables) || ndeltas < 0 || (ndeltas > 0 && !deltas))
     return set_err(ctx, RSB200_ERR_ARG, "dngop_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  std::unique_ptr<rsb200_plan, void (*)(rsb200_plan*)> holder(new rsb200_plan, rsb200_plan_destroy);
+  PlanHolder holder = new_plan(ctx, PlanKind::DngOp);
+  if (!holder)
+    return RSB200_ERR_CUDA;
   rsb200_plan* p = holder.get();
-  p->ctx = ctx;
-  p->kind = 8;
   p->nunits = njobs;
   std::vector<DngOpJobDev> hj((size_t)njobs);
   std::vector<DngOpDev> ho((size_t)nops);
-  p->pana_zero_slot.assign((size_t)nops, -1);
+  p->bad_slot.assign((size_t)nops, -1);
   uint64_t units = 0;
   if (const char* why = dngop_build(jobs, njobs, ops, nops, ntables, ndeltas, hj.data(), ho.data(),
-                                    p->pana_zero_slot.data(), &p->pana_zero_slots, &units))
+                                    p->bad_slot.data(), &p->nbad_slots, &units))
     return set_err(ctx, RSB200_ERR_ARG, "dngop plan: %s", why);
   for (int i = 0; i < njobs; ++i) {
     const uint64_t bytes = (uint64_t)(hj[i].row1 - hj[i].row0) * hj[i].samples * (jobs[i].is_f32 ? 4u : 2u);
@@ -933,26 +966,17 @@ extern "C" int rsb200_dngop_plan_create(rsb200_ctx* ctx, const rsb200_dngop_job*
   }
   p->dngop_njobs = njobs;
   p->dngop_units = (uint32_t)units;
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_dngop_jobs, sizeof(DngOpJobDev) * hj.size()));
-  CUDA_TRY(ctx, cudaMemcpy(p->d_dngop_jobs, hj.data(), sizeof(DngOpJobDev) * hj.size(),
-                           cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_dngop_ops, sizeof(DngOpDev) * (ho.size() + 1)));
-  if (!ho.empty())
-    CUDA_TRY(ctx, cudaMemcpy(p->d_dngop_ops, ho.data(), sizeof(DngOpDev) * ho.size(),
-                             cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_dngop_tables, sizeof(uint16_t) * 65536 * (size_t)(ntables + 1)));
-  if (ntables)
-    CUDA_TRY(ctx, cudaMemcpy(p->d_dngop_tables, tables, sizeof(uint16_t) * 65536 * (size_t)ntables,
-                             cudaMemcpyHostToDevice));
-  CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_dngop_deltas, sizeof(uint32_t) * (size_t)(ndeltas + 1)));
-  if (ndeltas)
-    CUDA_TRY(ctx, cudaMemcpy(p->d_dngop_deltas, deltas, sizeof(uint32_t) * (size_t)ndeltas,
-                             cudaMemcpyHostToDevice));
-  if (p->pana_zero_slots) {
-    CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_pana_zero_count, sizeof(uint32_t) * (size_t)p->pana_zero_slots));
-    CUDA_TRY(ctx, rsb_dev_alloc((void**)&p->d_pana_zero_list,
-                             sizeof(uint32_t) * (size_t)DNGOP_BAD_CAP * (size_t)p->pana_zero_slots));
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_dngop_jobs, hj.data(), sizeof(DngOpJobDev) * hj.size());
+  dev_upload(e, p->d_dngop_ops, ho.data(), sizeof(DngOpDev) * ho.size(), sizeof(DngOpDev));
+  dev_upload(e, p->d_dngop_tables, tables, sizeof(uint16_t) * 65536 * (size_t)ntables, sizeof(uint16_t) * 65536);
+  dev_upload(e, p->d_dngop_deltas, deltas, sizeof(uint32_t) * (size_t)ndeltas, sizeof(uint32_t));
+  if (p->nbad_slots) {
+    dev_alloc(e, p->d_bad_count, sizeof(uint32_t) * (size_t)p->nbad_slots);
+    dev_alloc(e, p->d_bad_list, sizeof(uint32_t) * (size_t)DNGOP_BAD_CAP * (size_t)p->nbad_slots);
   }
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "dngop plan upload failed: %s", cudaGetErrorString(e));
   p->launches_per_run = units ? 1 : 0;
   *out = holder.release();
   return RSB200_OK;
@@ -964,10 +988,10 @@ extern "C" int rsb200_scale_plan_create(rsb200_ctx* ctx, const rsb200_scale_job*
   if (!ctx || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "scale_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  std::unique_ptr<rsb200_plan, void (*)(rsb200_plan*)> holder(new rsb200_plan, rsb200_plan_destroy);
+  PlanHolder holder = new_plan(ctx, PlanKind::Scale);
+  if (!holder)
+    return RSB200_ERR_CUDA;
   rsb200_plan* p = holder.get();
-  p->ctx = ctx;
-  p->kind = 7;
   p->nunits = njobs;
   std::vector<ScaleJobDev> dev[2];
   uint32_t quads[2] = {0, 0};
@@ -1003,10 +1027,11 @@ extern "C" int rsb200_scale_plan_create(rsb200_ctx* ctx, const rsb200_scale_job*
       const uint32_t want = (uint32_t)((32ull * (uint64_t)ctx->sm_count + g.total_quads - 1) / std::max(g.total_quads, 1u));
       g.nseg = mode == 0 ? 1u : std::max(1u, std::min(std::min(want, 8u), std::max(1u, min_groups / 64u)));
     }
-    CUDA_TRY(ctx, rsb_dev_alloc((void**)&g.d_jobs, sizeof(ScaleJobDev) * dev[mode].size()));
-    p->scale_groups.push_back(g); // owned by the plan from here on
-    CUDA_TRY(ctx, cudaMemcpy(g.d_jobs, dev[mode].data(), sizeof(ScaleJobDev) * dev[mode].size(),
-                             cudaMemcpyHostToDevice));
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, dev[mode].data(), sizeof(ScaleJobDev) * dev[mode].size());
+    if (e != cudaSuccess)
+      return set_err(ctx, RSB200_ERR_CUDA, "scale plan upload failed: %s", cudaGetErrorString(e));
+    p->scale_groups.push_back(std::move(g));
   }
   p->launches_per_run = (int)p->scale_groups.size();
   *out = holder.release();
@@ -1018,11 +1043,10 @@ extern "C" int rsb200_sraw_plan_create(rsb200_ctx* ctx, const rsb200_sraw_job* j
   if (!ctx || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "sraw_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Sraw);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 3;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::map<std::pair<int, bool>, std::vector<SrawJobDev>> buckets;
   for (int i = 0; i < njobs; ++i) {
@@ -1035,10 +1059,8 @@ extern "C" int rsb200_sraw_plan_create(rsb200_ctx* ctx, const rsb200_sraw_job* j
                     (uint64_t)j.num_mcus * per * 2 <= j.in_pitch &&
                     (uint64_t)j.num_mcus * 12 <= j.out_pitch &&
                     (uint64_t)j.num_mcus * j.in_rows < 0xFFFF0000ull;
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "sraw job %d: malformed descriptor", i);
-    }
     SrawJobDev d;
     memset(&d, 0, sizeof d);
     d.in_offset = j.in_offset;
@@ -1070,24 +1092,18 @@ extern "C" int rsb200_sraw_plan_create(rsb200_ctx* ctx, const rsb200_sraw_job* j
       d.mcu_begin = (uint32_t)n;
       n += (uint64_t)d.num_mcus * d.in_rows;
     }
-    if (n >= 0xFFFF0000ull) {
-      rsb200_plan_destroy(p);
+    if (n >= 0xFFFF0000ull)
       return set_err(ctx, RSB200_ERR_ARG, "sraw plan: too many MCUs");
-    }
     g.total_mcus = (uint32_t)n;
     g.njobs = (int)kv.second.size();
-    cudaError_t e = rsb_dev_alloc(&g.d_jobs, sizeof(SrawJobDev) * kv.second.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(g.d_jobs, kv.second.data(), sizeof(SrawJobDev) * kv.second.size(),
-                     cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, kv.second.data(), sizeof(SrawJobDev) * kv.second.size());
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "sraw plan upload failed: %s", cudaGetErrorString(e));
-    }
-    p->sraw_groups.push_back(g);
+    p->sraw_groups.push_back(std::move(g));
   }
   p->launches_per_run = (int)p->sraw_groups.size();
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -1104,11 +1120,10 @@ extern "C" int rsb200_hasselblad_plan_create(rsb200_ctx* ctx, const rsb200_huff_
   for (int i = 0; i < ntables; ++i)
     if (!build_dev_table(tables[i], ht[(size_t)i]))
       return set_err(ctx, RSB200_ERR_ARG, "huffman table %d is malformed", i);
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Hasselblad);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 11;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::vector<DevHassJob> dj((size_t)njobs);
   std::vector<DevHassCta> ctas;
@@ -1120,10 +1135,8 @@ extern "C" int rsb200_hasselblad_plan_create(rsb200_ctx* ctx, const rsb200_huff_
     const bool ok = j.width > 0 && j.height > 0 && j.width % 2 == 0 && j.width <= 12000 && j.height <= 8842 &&
                     (j.in_offset % 4) == 0 && j.in_size < (1u << 28) && (j.out_offset % 4) == 0 &&
                     (j.out_pitch % 4) == 0 && (uint64_t)j.width * 2 <= j.out_pitch && j.table < ntables;
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "hasselblad job %d: malformed descriptor", i);
-    }
     DevHassJob& d = dj[(size_t)i];
     memset(&d, 0, sizeof d);
     d.in_offset = j.in_offset;
@@ -1153,46 +1166,31 @@ extern "C" int rsb200_hasselblad_plan_create(rsb200_ctx* ctx, const rsb200_huff_
                                                                             (uint64_t)j.width * 2));
   }
   row_begin[(size_t)njobs] = (uint32_t)rows_total;
-  if (nseg_total >= 0x7FFFFFFFull || rows_total >= 0x7FFFFFFull) {
-    delete p;
+  if (nseg_total >= 0x7FFFFFFFull || rows_total >= 0x7FFFFFFull)
     return set_err(ctx, RSB200_ERR_ARG, "hasselblad plan: too large");
-  }
   p->hass_nseg = (uint32_t)nseg_total;
   p->hass_ncta = (uint32_t)ctas.size();
   p->hass_rows = (uint32_t)rows_total;
   p->ntables = ntables;
   cudaError_t e = cudaSuccess;
-  auto up = [&](void** dptr, const void* src, size_t bytes) {
-    if (e != cudaSuccess)
-      return;
-    e = rsb_dev_alloc(dptr, bytes ? bytes : 16);
-    if (e == cudaSuccess && bytes)
-      e = cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice);
-  };
-  up((void**)&p->d_tables, ht.data(), sizeof(DevTable) * ht.size());
-  up((void**)&p->d_hass_jobs, dj.data(), sizeof(DevHassJob) * dj.size());
-  up((void**)&p->d_hass_ctas, ctas.data(), sizeof(DevHassCta) * ctas.size());
-  up((void**)&p->d_hass_seg_job, seg_job.data(), sizeof(uint32_t) * seg_job.size());
-  up((void**)&p->d_hass_row_begin, row_begin.data(), sizeof(uint32_t) * row_begin.size());
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_hass_u32,
-                      sizeof(uint32_t) * (4ull * nseg_total + 2ull * ctas.size() + H_ROUNDS + 8));
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_hass_states, sizeof(DevHassState) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_host_alloc((void**)&p->h_hass_states, sizeof(DevHassState) * (size_t)njobs);
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  dev_upload(e, p->d_tables, ht.data(), sizeof(DevTable) * ht.size());
+  dev_upload(e, p->d_hass_jobs, dj.data(), sizeof(DevHassJob) * dj.size());
+  dev_upload(e, p->d_hass_ctas, ctas.data(), sizeof(DevHassCta) * ctas.size());
+  dev_upload(e, p->d_hass_seg_job, seg_job.data(), sizeof(uint32_t) * seg_job.size());
+  dev_upload(e, p->d_hass_row_begin, row_begin.data(), sizeof(uint32_t) * row_begin.size());
+  dev_alloc(e, p->d_hass_u32, sizeof(uint32_t) * (4ull * nseg_total + 2ull * ctas.size() + H_ROUNDS + 8));
+  dev_alloc(e, p->d_hass_states, sizeof(DevHassState) * (size_t)njobs);
+  host_alloc(e, p->h_hass_states, sizeof(DevHassState) * (size_t)njobs);
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "hasselblad plan allocation failed: %s", cudaGetErrorString(e));
-  }
   p->launches_per_run = 1 + 2 * H_ROUNDS + 1 + 2 + 1 + 1;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
 static cudaError_t run_hasselblad(const rsb200_plan* p, const uint8_t* in, uint8_t* outp, cudaStream_t st) {
   const uint32_t n = p->hass_nseg, nc = p->hass_ncta;
-  uint32_t* start = p->d_hass_u32;
+  uint32_t* start = p->d_hass_u32.get();
   uint32_t* parsed = start + n;
   uint32_t* exitp = parsed + n;
   uint32_t* count = exitp + n;
@@ -1201,22 +1199,22 @@ static cudaError_t run_hasselblad(const rsb200_plan* p, const uint8_t* in, uint8
   uint32_t* changed = cta_base + nc;
   const size_t smem = sizeof(HassShared);
   const uint32_t nb = (std::max<uint32_t>(std::max<uint32_t>(n, (uint32_t)p->nunits), H_ROUNDS + 1) + 255) / 256;
-  hass_init_kernel<<<nb, 256, 0, st>>>(p->d_hass_jobs, p->nunits, n, p->d_hass_seg_job, start, parsed,
-                                       p->d_hass_states, changed);
+  hass_init_kernel<<<nb, 256, 0, st>>>(p->d_hass_jobs.get(), p->nunits, n, p->d_hass_seg_job.get(), start, parsed,
+                                       p->d_hass_states.get(), changed);
   for (int r = 0; r < H_ROUNDS; ++r) {
-    hass_parse_kernel<<<nc, H_NT, smem, st>>>(in, p->d_hass_jobs, p->d_tables, p->d_hass_ctas, start, parsed,
+    hass_parse_kernel<<<nc, H_NT, smem, st>>>(in, p->d_hass_jobs.get(), p->d_tables.get(), p->d_hass_ctas.get(), start, parsed,
                                               exitp, count);
-    hass_link_kernel<<<(n + 255) / 256, 256, 0, st>>>(p->d_hass_jobs, p->nunits, n, p->d_hass_seg_job, start,
+    hass_link_kernel<<<(n + 255) / 256, 256, 0, st>>>(p->d_hass_jobs.get(), p->nunits, n, p->d_hass_seg_job.get(), start,
                                                       exitp, changed + r);
   }
-  hass_serial_kernel<<<p->nunits, 32, 0, st>>>(in, p->d_hass_jobs, p->d_tables, start, parsed, exitp, count,
+  hass_serial_kernel<<<p->nunits, 32, 0, st>>>(in, p->d_hass_jobs.get(), p->d_tables.get(), start, parsed, exitp, count,
                                                changed + (H_ROUNDS - 1));
-  hass_ctasum_kernel<<<nc, H_NT, smem, st>>>(p->d_hass_jobs, p->d_hass_ctas, count, cta_sum);
-  hass_ctascan_kernel<<<(p->nunits + 63) / 64, 64, 0, st>>>(p->d_hass_jobs, p->nunits, cta_sum, cta_base);
-  hass_decode_kernel<<<nc, H_NT, smem, st>>>(in, p->d_hass_jobs, p->d_tables, p->d_hass_ctas, start, exitp,
-                                             count, cta_base, outp, p->d_hass_states);
-  hass_rows_kernel<<<(p->hass_rows * 32 + 255) / 256, 256, 0, st>>>(p->d_hass_jobs, p->nunits,
-                                                                   p->d_hass_row_begin, outp);
+  hass_ctasum_kernel<<<nc, H_NT, smem, st>>>(p->d_hass_jobs.get(), p->d_hass_ctas.get(), count, cta_sum);
+  hass_ctascan_kernel<<<(p->nunits + 63) / 64, 64, 0, st>>>(p->d_hass_jobs.get(), p->nunits, cta_sum, cta_base);
+  hass_decode_kernel<<<nc, H_NT, smem, st>>>(in, p->d_hass_jobs.get(), p->d_tables.get(), p->d_hass_ctas.get(), start, exitp,
+                                             count, cta_base, outp, p->d_hass_states.get());
+  hass_rows_kernel<<<(p->hass_rows * 32 + 255) / 256, 256, 0, st>>>(p->d_hass_jobs.get(), p->nunits,
+                                                                   p->d_hass_row_begin.get(), outp);
   return cudaGetLastError();
 }
 
@@ -1237,11 +1235,10 @@ extern "C" int rsb200_phaseone_plan_create(rsb200_ctx* ctx, const rsb200_phaseon
   if (!ctx || !jobs || njobs <= 0 || !strips || nstrips <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "phaseone_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::PhaseOne);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 6;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::vector<P1JobDev> dj((size_t)njobs);
   std::vector<P1StripDev> ds;
@@ -1269,10 +1266,8 @@ extern "C" int rsb200_phaseone_plan_create(rsb200_ctx* ctx, const rsb200_phaseon
         p->need_in = std::max<uint64_t>(p->need_in, sat_add(st.in_offset, st.in_size));
       }
     }
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "phaseone job %d: malformed descriptor or strips", i);
-    }
     dj[(size_t)i].out_offset = j.out_offset;
     dj[(size_t)i].out_pitch = j.out_pitch;
     dj[(size_t)i].width = j.width;
@@ -1284,55 +1279,45 @@ extern "C" int rsb200_phaseone_plan_create(rsb200_ctx* ctx, const rsb200_phaseon
   p->p1_nstrips = (uint32_t)ds.size();
   for (int i = 0; i < njobs; ++i)
     p->p1_gstride = std::max<uint32_t>(p->p1_gstride, (jobs[i].width / 8u + 1u + 3u) & ~3u); // (16-byte rows)
-  cudaError_t e = rsb_dev_alloc((void**)&p->d_p1_strips, sizeof(P1StripDev) * ds.size());
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_p1_gdesc, sizeof(uint32_t) * (size_t)p->p1_gstride * ds.size());
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_p1_rowflag, sizeof(uint32_t) * ds.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_p1_strips, ds.data(), sizeof(P1StripDev) * ds.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_p1_jobs, sizeof(P1JobDev) * dj.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_p1_jobs, dj.data(), sizeof(P1JobDev) * dj.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw2_bad, sizeof(uint32_t) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_host_alloc((void**)&p->h_arw2_bad, sizeof(uint32_t) * (size_t)njobs);
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_p1_strips, ds.data(), sizeof(P1StripDev) * ds.size());
+  dev_alloc(e, p->d_p1_gdesc, sizeof(uint32_t) * (size_t)p->p1_gstride * ds.size());
+  dev_alloc(e, p->d_p1_rowflag, sizeof(uint32_t) * ds.size());
+  dev_upload(e, p->d_p1_jobs, dj.data(), sizeof(P1JobDev) * dj.size());
+  dev_alloc(e, p->d_job_bad, sizeof(uint32_t) * (size_t)njobs);
+  host_alloc(e, p->h_job_bad, sizeof(uint32_t) * (size_t)njobs);
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "phaseone plan upload failed: %s", cudaGetErrorString(e));
-  }
   p->p1_ver = p1_version();
   {
     const char* e = getenv("RSB200_P1W");
     p->p1_walk1 = (e && e[0] >= '1' && e[0] <= '8' && !e[1]) ? e[0] - '0' : 0;
   }
   p->launches_per_run = p->p1_ver == 3 ? 2 : 1;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
 static cudaError_t run_phaseone(const rsb200_plan* p, const uint8_t* in, uint8_t* outp,
                                 cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(p->d_arw2_bad, 0, sizeof(uint32_t) * (size_t)p->nunits, st);
+  cudaError_t e = cudaMemsetAsync(p->d_job_bad.get(), 0, sizeof(uint32_t) * (size_t)p->nunits, st);
   if (e != cudaSuccess)
     return e;
   const int v = p->p1_ver;
   const uint32_t nb = (p->p1_nstrips + P1_NT - 1) / P1_NT;
   if (v == 1) {
-    p1_kernel<<<nb, P1_NT, 0, st>>>(in, outp, p->d_p1_strips, p->p1_nstrips, p->d_p1_jobs,
-                                    p->d_arw2_bad);
+    p1_kernel<<<nb, P1_NT, 0, st>>>(in, outp, p->d_p1_strips.get(), p->p1_nstrips, p->d_p1_jobs.get(),
+                                    p->d_job_bad.get());
   } else if (v == 2) {
-    p1_kernel_v2<<<nb, P1_NT, 0, st>>>(in, outp, p->d_p1_strips, p->p1_nstrips, p->d_p1_jobs,
-                                       p->d_arw2_bad);
+    p1_kernel_v2<<<nb, P1_NT, 0, st>>>(in, outp, p->d_p1_strips.get(), p->p1_nstrips, p->d_p1_jobs.get(),
+                                       p->d_job_bad.get());
   } else {
     p1_walk_kernel<<<(p->p1_nstrips + P1W_NT - 1) / P1W_NT, P1W_NT, 0, st>>>(
-        in, p->d_p1_strips, p->p1_nstrips, p->d_p1_jobs, p->p1_gstride, p->d_p1_gdesc, p->d_p1_rowflag,
+        in, p->d_p1_strips.get(), p->p1_nstrips, p->d_p1_jobs.get(), p->p1_gstride, p->d_p1_gdesc.get(), p->d_p1_rowflag.get(),
         p->p1_walk1);
     p1_decode_kernel<<<(p->p1_nstrips * 32u + P1D_NT - 1) / P1D_NT, P1D_NT, 0, st>>>(
-        in, outp, p->d_p1_strips, p->p1_nstrips, p->d_p1_jobs, p->p1_gstride, p->d_p1_gdesc,
-        p->d_p1_rowflag, p->d_arw2_bad);
+        in, outp, p->d_p1_strips.get(), p->p1_nstrips, p->d_p1_jobs.get(), p->p1_gstride, p->d_p1_gdesc.get(),
+        p->d_p1_rowflag.get(), p->d_job_bad.get());
   }
   return cudaGetLastError();
 }
@@ -1361,11 +1346,10 @@ extern "C" int rsb200_samsung0_plan_create(rsb200_ctx* ctx, const rsb200_samsung
     if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "samsung0 job %d: malformed descriptor or strips", i);
   }
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::SamsungV0);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 12;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::vector<S0JobDev> dj((size_t)njobs);
   std::vector<S0RowDev> dr;
@@ -1405,69 +1389,53 @@ extern "C" int rsb200_samsung0_plan_create(rsb200_ctx* ctx, const rsb200_samsung
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch +
                                                       2ull * j.width));
   }
-  if (nodes >= S0_ROOT) {
-    delete p;
+  if (nodes >= S0_ROOT)
     return set_err(ctx, RSB200_ERR_ARG, "samsung0 plan: too many frames for one plan");
-  }
   p->s0_nrows = (uint32_t)dr.size();
   p->s0_nnodes = (uint32_t)nodes;
   while ((1u << p->s0_rounds) < depth)
     ++p->s0_rounds;
-  cudaError_t e = rsb_dev_alloc(&p->d_s0_rows, sizeof(S0RowDev) * dr.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_s0_rows, dr.data(), sizeof(S0RowDev) * dr.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_jobs, sizeof(S0JobDev) * dj.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_s0_jobs, dj.data(), sizeof(S0JobDev) * dj.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_desc, sizeof(uint2) * blk);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_adj, sizeof(uint16_t) * px);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_nodes, sizeof(uint2) * 2 * nodes);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_carry, sizeof(uint32_t) * carry);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_rowfail, sizeof(uint32_t) * dr.size());
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_jobfail, sizeof(uint32_t) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_res, sizeof(uint2) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_host_alloc((void**)&p->h_s0_res, sizeof(uint2) * (size_t)njobs);
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_s0_rows, dr.data(), sizeof(S0RowDev) * dr.size());
+  dev_upload(e, p->d_s0_jobs, dj.data(), sizeof(S0JobDev) * dj.size());
+  dev_alloc(e, p->d_s0_desc, sizeof(uint2) * blk);
+  dev_alloc(e, p->d_s0_adj, sizeof(uint16_t) * px);
+  dev_alloc(e, p->d_s0_nodes, sizeof(uint2) * 2 * nodes);
+  dev_alloc(e, p->d_s0_carry, sizeof(uint32_t) * carry);
+  dev_alloc(e, p->d_s0_rowfail, sizeof(uint32_t) * dr.size());
+  dev_alloc(e, p->d_s0_jobfail, sizeof(uint32_t) * (size_t)njobs);
+  dev_alloc(e, p->d_job_res, sizeof(uint2) * (size_t)njobs);
+  host_alloc(e, p->h_job_res, sizeof(uint2) * (size_t)njobs);
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "samsung0 plan allocation failed: %s", cudaGetErrorString(e));
-  }
   p->launches_per_run = 6 + p->s0_rounds;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
 static cudaError_t run_samsung0(const rsb200_plan* p, const uint8_t* in, uint8_t* outp, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(p->d_s0_jobfail, 0xFF, sizeof(uint32_t) * (size_t)p->nunits, st);
+  cudaError_t e = cudaMemsetAsync(p->d_s0_jobfail.get(), 0xFF, sizeof(uint32_t) * (size_t)p->nunits, st);
   if (e != cudaSuccess)
     return e;
   const uint32_t nj = (uint32_t)p->nunits;
   s0_walk_kernel<<<(p->s0_nrows + S0W_NT - 1) / S0W_NT, S0W_NT, 0, st>>>(
-      in, p->d_s0_rows, p->s0_nrows, p->d_s0_jobs, p->d_s0_desc, p->d_s0_rowfail, p->d_s0_jobfail);
+      in, p->d_s0_rows.get(), p->s0_nrows, p->d_s0_jobs.get(), p->d_s0_desc.get(), p->d_s0_rowfail.get(), p->d_s0_jobfail.get());
   s0_diff_kernel<<<(p->s0_nrows + S0D_NT / 32 - 1) / (S0D_NT / 32), S0D_NT, 0, st>>>(
-      in, p->d_s0_rows, p->s0_nrows, p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj);
+      in, p->d_s0_rows.get(), p->s0_nrows, p->d_s0_jobs.get(), p->d_s0_desc.get(), p->d_s0_adj.get());
   s0_node_kernel<<<dim3((p->s0_max_nodes + S0N_NT - 1) / S0N_NT, nj), S0N_NT, 0, st>>>(
-      p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, p->d_s0_nodes);
-  uint2* src = p->d_s0_nodes;
-  uint2* dst = p->d_s0_nodes + p->s0_nnodes;
+      p->d_s0_jobs.get(), p->d_s0_desc.get(), p->d_s0_adj.get(), p->d_s0_nodes.get());
+  uint2* src = p->d_s0_nodes.get();
+  uint2* dst = p->d_s0_nodes.get() + p->s0_nnodes;
   for (int r = 0; r < p->s0_rounds; ++r) {
     s0_jump_kernel<<<(p->s0_nnodes + S0N_NT - 1) / S0N_NT, S0N_NT, 0, st>>>(src, dst, p->s0_nnodes);
     std::swap(src, dst);
   }
   const dim3 tiles((p->s0_max_w + S0C_NT - 1) / S0C_NT, p->s0_max_tiles, nj);
-  s0_scan_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, src, p->d_s0_carry);
-  s0_carry_kernel<<<dim3((2 * p->s0_max_w + S0C_NT - 1) / S0C_NT, nj), S0C_NT, 0, st>>>(p->d_s0_jobs,
-                                                                                     p->d_s0_carry);
-  s0_store_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs, p->d_s0_desc, p->d_s0_adj, src, p->d_s0_carry,
-                                            p->d_s0_rowfail, p->d_s0_jobfail, outp, p->d_s0_res);
+  s0_scan_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs.get(), p->d_s0_desc.get(), p->d_s0_adj.get(), src, p->d_s0_carry.get());
+  s0_carry_kernel<<<dim3((2 * p->s0_max_w + S0C_NT - 1) / S0C_NT, nj), S0C_NT, 0, st>>>(p->d_s0_jobs.get(),
+                                                                                     p->d_s0_carry.get());
+  s0_store_kernel<<<tiles, S0C_NT, 0, st>>>(p->d_s0_jobs.get(), p->d_s0_desc.get(), p->d_s0_adj.get(), src, p->d_s0_carry.get(),
+                                            p->d_s0_rowfail.get(), p->d_s0_jobfail.get(), outp, p->d_job_res.get());
   return cudaGetLastError();
 }
 
@@ -1502,11 +1470,10 @@ extern "C" int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung
         j.reserved)
       return set_err(ctx, RSB200_ERR_ARG, "samsung2 job %d: malformed descriptor", i);
   }
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::SamsungV2);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 13;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::vector<S2FrameDev> fr((size_t)njobs);
   std::vector<uint32_t> starts((size_t)njobs * 4);
@@ -1516,10 +1483,8 @@ extern "C" int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung
     S2FrameDev& f = fr[(size_t)i];
     s2_place_frame(f, t, starts.data(), (uint32_t)njobs, (uint32_t)i, j.in_offset, j.in_size, j.header, j.bits,
                    (uint32_t)j.width, (uint32_t)j.height, j.out_offset, j.out_pitch);
-    if (t.tab >= (1ull << 31) || t.rows >= (1ull << 31)) {
-      delete p;
+    if (t.tab >= (1ull << 31) || t.rows >= (1ull << 31))
       return set_err(ctx, RSB200_ERR_ARG, "samsung2 plan: too many frames for one plan");
-    }
     p->in_bytes += j.in_size;
     p->out_bytes += (uint64_t)f.w * f.h * 2;
     p->pixels += (uint64_t)f.w * f.h;
@@ -1531,67 +1496,51 @@ extern "C" int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung
   p->s2_njump = (uint32_t)jump;
   p->s2_nrows = (uint32_t)rows;
   p->s2_ncp = (uint32_t)cps;
-  cudaError_t e = rsb_dev_alloc(&p->d_s2_frames, sizeof(S2FrameDev) * fr.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_s2_frames, fr.data(), sizeof(S2FrameDev) * fr.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_starts, sizeof(uint32_t) * starts.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_s2_starts, starts.data(), sizeof(uint32_t) * starts.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_tab, sizeof(uint32_t) * tab);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_jump, sizeof(uint32_t) * 2 * jump);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_rowstart, sizeof(uint32_t) * rows);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_cp, sizeof(uint32_t) * cps);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_ncp, sizeof(uint32_t) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_fail, sizeof(uint2) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_desc, sizeof(uint2) * desc);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s2_px, sizeof(int16_t) * px);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc(&p->d_s0_res, sizeof(uint2) * (size_t)njobs);
-  if (e == cudaSuccess)
-    e = rsb_host_alloc((void**)&p->h_s0_res, sizeof(uint2) * (size_t)njobs);
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_s2_frames, fr.data(), sizeof(S2FrameDev) * fr.size());
+  dev_upload(e, p->d_s2_starts, starts.data(), sizeof(uint32_t) * starts.size());
+  dev_alloc(e, p->d_s2_tab, sizeof(uint32_t) * tab);
+  dev_alloc(e, p->d_s2_jump, sizeof(uint32_t) * 2 * jump);
+  dev_alloc(e, p->d_s2_rowstart, sizeof(uint32_t) * rows);
+  dev_alloc(e, p->d_s2_cp, sizeof(uint32_t) * cps);
+  dev_alloc(e, p->d_s2_ncp, sizeof(uint32_t) * (size_t)njobs);
+  dev_alloc(e, p->d_s2_fail, sizeof(uint2) * (size_t)njobs);
+  dev_alloc(e, p->d_s2_desc, sizeof(uint2) * desc);
+  dev_alloc(e, p->d_s2_px, sizeof(int16_t) * px);
+  dev_alloc(e, p->d_job_res, sizeof(uint2) * (size_t)njobs);
+  host_alloc(e, p->h_job_res, sizeof(uint2) * (size_t)njobs);
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "samsung2 plan allocation failed: %s", cudaGetErrorString(e));
-  }
   p->launches_per_run = 7 + S2_JUMP;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
 static cudaError_t run_samsung2(const rsb200_plan* p, const uint8_t* in, uint8_t* outp, cudaStream_t st) {
   const uint32_t nf = (uint32_t)p->nunits;
-  const uint32_t* s = p->d_s2_starts;
-  s2_cand_kernel<<<(p->s2_ntab + S2W_NT - 1) / S2W_NT, S2W_NT, 0, st>>>(in, p->d_s2_frames, s, nf, p->s2_ntab,
-                                                                         p->d_s2_tab);
-  uint32_t* src = p->d_s2_jump;
-  uint32_t* dst = p->d_s2_jump + p->s2_njump;
+  const uint32_t* s = p->d_s2_starts.get();
+  s2_cand_kernel<<<(p->s2_ntab + S2W_NT - 1) / S2W_NT, S2W_NT, 0, st>>>(in, p->d_s2_frames.get(), s, nf, p->s2_ntab,
+                                                                         p->d_s2_tab.get());
+  uint32_t* src = p->d_s2_jump.get();
+  uint32_t* dst = p->d_s2_jump.get() + p->s2_njump;
   const uint32_t gj = (p->s2_njump + S2J_NT - 1) / S2J_NT;
-  s2_pair_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames, s + nf, nf, p->s2_njump, p->d_s2_tab, src);
+  s2_pair_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames.get(), s + nf, nf, p->s2_njump, p->d_s2_tab.get(), src);
   for (int r = 0; r < S2_JUMP; ++r) {
-    s2_double_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames, s + nf, nf, p->s2_njump, src, dst);
+    s2_double_kernel<<<gj, S2J_NT, 0, st>>>(p->d_s2_frames.get(), s + nf, nf, p->s2_njump, src, dst);
     std::swap(src, dst);
   }
-  s2_coarse_kernel<<<(nf + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames, nf, p->d_s2_tab, src,
-                                                                   p->d_s2_rowstart, p->d_s2_cp, p->d_s2_ncp,
-                                                                   p->d_s2_fail);
-  s2_fine_kernel<<<(p->s2_ncp + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames, s + 3 * nf, nf, p->s2_ncp,
-                                                                        p->d_s2_tab, p->d_s2_cp, p->d_s2_ncp,
-                                                                        p->d_s2_rowstart, p->d_s2_fail);
+  s2_coarse_kernel<<<(nf + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames.get(), nf, p->d_s2_tab.get(), src,
+                                                                   p->d_s2_rowstart.get(), p->d_s2_cp.get(), p->d_s2_ncp.get(),
+                                                                   p->d_s2_fail.get());
+  s2_fine_kernel<<<(p->s2_ncp + S2J_NT - 1) / S2J_NT, S2J_NT, 0, st>>>(p->d_s2_frames.get(), s + 3 * nf, nf, p->s2_ncp,
+                                                                        p->d_s2_tab.get(), p->d_s2_cp.get(), p->d_s2_ncp.get(),
+                                                                        p->d_s2_rowstart.get(), p->d_s2_fail.get());
   s2_desc_kernel<<<(p->s2_nrows + S2W_NT - 1) / S2W_NT, S2W_NT, 0, st>>>(
-      in, p->d_s2_frames, s + 2 * nf, nf, p->s2_nrows, p->d_s2_rowstart, p->d_s2_fail, p->d_s2_desc);
-  s2_diff_kernel<<<p->s2_nrows, S2X_NT, 0, st>>>(in, p->d_s2_frames, s + 2 * nf, nf, p->d_s2_fail, p->d_s2_desc,
-                                                 p->d_s2_px);
-  s2_recon_kernel<<<nf, S2R_NT, 0, st>>>(p->d_s2_frames, p->d_s2_fail, p->d_s2_desc, p->d_s2_px, outp,
-                                         p->d_s0_res);
+      in, p->d_s2_frames.get(), s + 2 * nf, nf, p->s2_nrows, p->d_s2_rowstart.get(), p->d_s2_fail.get(), p->d_s2_desc.get());
+  s2_diff_kernel<<<p->s2_nrows, S2X_NT, 0, st>>>(in, p->d_s2_frames.get(), s + 2 * nf, nf, p->d_s2_fail.get(), p->d_s2_desc.get(),
+                                                 p->d_s2_px.get());
+  s2_recon_kernel<<<nf, S2R_NT, 0, st>>>(p->d_s2_frames.get(), p->d_s2_fail.get(), p->d_s2_desc.get(), p->d_s2_px.get(), outp,
+                                         p->d_job_res.get());
   return cudaGetLastError();
 }
 
@@ -1603,11 +1552,10 @@ extern "C" int rsb200_pana_plan_create(rsb200_ctx* ctx, const rsb200_pana_job* j
   if (!ctx || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "pana_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Pana);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 5;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::map<std::pair<int, int>, std::vector<PanaJobDev>> buckets;
   for (int i = 0; i < njobs; ++i) {
@@ -1631,10 +1579,8 @@ extern "C" int rsb200_pana_plan_create(rsb200_ctx* ctx, const rsb200_pana_job* j
                     (uint64_t)j.width * 2 <= j.out_pitch && area < 0xFFFF0000ull &&
                     (j.version != 4 || (j.section_split_offset <= 0x4000u && j.width <= 0xFFFFu &&
                                         j.height <= 0xFFFFu));
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "pana job %d: malformed descriptor", i);
-    }
     PanaJobDev d;
     memset(&d, 0, sizeof d);
     d.in_offset = j.in_offset;
@@ -1643,12 +1589,12 @@ extern "C" int rsb200_pana_plan_create(rsb200_ctx* ctx, const rsb200_pana_job* j
     d.width = j.width;
     d.height = j.height;
     d.units = (uint32_t)units;
-    p->pana_zero_slot.push_back(-1);
+    p->bad_slot.push_back(-1);
     if (j.version == 4) {
       d.split = j.section_split_offset;
       if (!j.zero_is_not_bad) {
-        p->pana_zero_slot.back() = p->pana_zero_slots;
-        d.zero_slot = (uint32_t)++p->pana_zero_slots;
+        p->bad_slot.back() = p->nbad_slots;
+        d.zero_slot = (uint32_t)++p->nbad_slots;
       }
     }
     buckets[{(int)j.version, bps}].push_back(d);
@@ -1668,34 +1614,25 @@ extern "C" int rsb200_pana_plan_create(rsb200_ctx* ctx, const rsb200_pana_job* j
       d.unit_begin = (uint32_t)n;
       n += d.units;
     }
-    if (n >= 0xFFFF0000ull) {
-      rsb200_plan_destroy(p);
+    if (n >= 0xFFFF0000ull)
       return set_err(ctx, RSB200_ERR_ARG, "pana plan: too many blocks");
-    }
     g.total_units = (uint32_t)n;
     g.njobs = (int)kv.second.size();
-    cudaError_t e = rsb_dev_alloc(&g.d_jobs, sizeof(PanaJobDev) * kv.second.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(g.d_jobs, kv.second.data(), sizeof(PanaJobDev) * kv.second.size(),
-                     cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    cudaError_t e = cudaSuccess;
+    dev_upload(e, g.d_jobs, kv.second.data(), sizeof(PanaJobDev) * kv.second.size());
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "pana plan upload failed: %s", cudaGetErrorString(e));
-    }
-    p->pana_groups.push_back(g);
+    p->pana_groups.push_back(std::move(g));
   }
-  if (p->pana_zero_slots) {
-    cudaError_t e = rsb_dev_alloc(&p->d_pana_zero_count, sizeof(uint32_t) * (size_t)p->pana_zero_slots);
-    if (e == cudaSuccess)
-      e = rsb_dev_alloc(&p->d_pana_zero_list,
-                     sizeof(uint32_t) * (size_t)PANA_ZERO_CAP * (size_t)p->pana_zero_slots);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+  if (p->nbad_slots) {
+    cudaError_t e = cudaSuccess;
+    dev_alloc(e, p->d_bad_count, sizeof(uint32_t) * (size_t)p->nbad_slots);
+    dev_alloc(e, p->d_bad_list, sizeof(uint32_t) * (size_t)PANA_ZERO_CAP * (size_t)p->nbad_slots);
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "pana plan: bad-pixel lists: %s", cudaGetErrorString(e));
-    }
   }
   p->launches_per_run = (int)p->pana_groups.size();
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -1705,12 +1642,12 @@ static cudaError_t run_pana_group(const rsb200_plan* p, const PanaGroup& g, cons
                                   uint8_t* outp, cudaStream_t st) {
   const uint32_t nb = (g.total_units + PANA_NT - 1) / PANA_NT;
 #define RSB_PANA(V, B)                                                                     \
-  pana_kernel<V, B><<<nb, PANA_NT, 0, st>>>(in, outp, g.d_jobs, g.njobs, g.total_units,    \
-                                            p->d_pana_zero_count, p->d_pana_zero_list)
+  pana_kernel<V, B><<<nb, PANA_NT, 0, st>>>(in, outp, g.d_jobs.get(), g.njobs, g.total_units,    \
+                                            p->d_bad_count.get(), p->d_bad_list.get())
   if (g.version == 4) {
-    if (p->pana_zero_slots) {
-      const cudaError_t e = cudaMemsetAsync(p->d_pana_zero_count, 0,
-                                            sizeof(uint32_t) * (size_t)p->pana_zero_slots, st);
+    if (p->nbad_slots) {
+      const cudaError_t e = cudaMemsetAsync(p->d_bad_count.get(), 0,
+                                            sizeof(uint32_t) * (size_t)p->nbad_slots, st);
       if (e != cudaSuccess)
         return e;
     }
@@ -1738,11 +1675,10 @@ extern "C" int rsb200_arw2_plan_create(rsb200_ctx* ctx, const rsb200_arw2_job* j
   if (!ctx || !jobs || njobs <= 0 || !out || ntables < 0 || (ntables > 0 && !tables))
     return set_err(ctx, RSB200_ERR_ARG, "arw2_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Arw2);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
-  p->kind = 4;
+  rsb200_plan* p = holder.get();
   p->nunits = njobs;
   std::vector<Arw2JobDev> dev((size_t)njobs);
   uint64_t groups = 0;
@@ -1753,10 +1689,8 @@ extern "C" int rsb200_arw2_plan_create(rsb200_ctx* ctx, const rsb200_arw2_job* j
     const bool ok = j.width > 0 && j.height > 0 && j.width % 32 == 0 && j.width <= 9600 &&
                     j.height <= 6376 && (j.out_offset % 16) == 0 && (j.out_pitch % 16) == 0 &&
                     (uint64_t)j.width * 2 <= j.out_pitch && j.table < ntables;
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "arw2 job %d: malformed descriptor", i);
-    }
     (j.table >= 0 ? any_table : any_plain) = true;
     Arw2JobDev& d = dev[(size_t)i];
     d.in_offset = j.in_offset;
@@ -1776,14 +1710,10 @@ extern "C" int rsb200_arw2_plan_create(rsb200_ctx* ctx, const rsb200_arw2_job* j
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch +
                                                       2ull * j.width));
   }
-  if (any_table && any_plain) {
-    delete p;
+  if (any_table && any_plain)
     return set_err(ctx, RSB200_ERR_ARG, "arw2 plan: jobs with and without a table cannot be mixed");
-  }
-  if (groups >= 0xFFFF0000ull) {
-    delete p;
+  if (groups >= 0xFFFF0000ull)
     return set_err(ctx, RSB200_ERR_ARG, "arw2 plan: too many blocks");
-  }
   p->arw2_groups = (uint32_t)groups;
   p->arw2_mode = !any_table ? 0 : (dither ? 2 : 1);
   p->arw2_ntables = any_table ? ntables : 0;
@@ -1807,41 +1737,29 @@ extern "C" int rsb200_arw2_plan_create(rsb200_ctx* ctx, const rsb200_arw2_job* j
       v = v * step % ARW2_M;
     }
     cudaError_t e = cudaMemcpyToSymbol(c_arw2_jump, jump, sizeof jump);
-    if (e == cudaSuccess)
-      e = rsb_dev_alloc(&p->d_arw2_jobs, sizeof(Arw2JobDev) * dev.size());
-    if (e == cudaSuccess)
-      e = cudaMemcpy(p->d_arw2_jobs, dev.data(), sizeof(Arw2JobDev) * dev.size(),
-                     cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = rsb_dev_alloc(&p->d_arw2_tables, tcut.size() * sizeof(uint16_t) + 16);
-    if (e == cudaSuccess && !tcut.empty())
-      e = cudaMemcpy(p->d_arw2_tables, tcut.data(), tcut.size() * sizeof(uint16_t),
-                     cudaMemcpyHostToDevice);
-    if (e == cudaSuccess)
-      e = rsb_dev_alloc(&p->d_arw2_bad, sizeof(uint32_t) * (size_t)njobs);
-    if (e == cudaSuccess)
-      e = rsb_host_alloc((void**)&p->h_arw2_bad, sizeof(uint32_t) * (size_t)njobs);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
+    dev_upload(e, p->d_arw2_jobs, dev.data(), sizeof(Arw2JobDev) * dev.size());
+    dev_upload(e, p->d_arw2_tables, tcut.data(), tcut.size() * sizeof(uint16_t), 16);
+    dev_alloc(e, p->d_job_bad, sizeof(uint32_t) * (size_t)njobs);
+    host_alloc(e, p->h_job_bad, sizeof(uint32_t) * (size_t)njobs);
+    if (e != cudaSuccess)
       return set_err(ctx, RSB200_ERR_CUDA, "arw2 plan upload failed: %s", cudaGetErrorString(e));
-    }
   }
   p->launches_per_run = 1;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
 static cudaError_t run_arw2(const rsb200_plan* p, const uint8_t* in, uint8_t* outp,
                             cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(p->d_arw2_bad, 0, sizeof(uint32_t) * (size_t)p->nunits, st);
+  cudaError_t e = cudaMemsetAsync(p->d_job_bad.get(), 0, sizeof(uint32_t) * (size_t)p->nunits, st);
   if (e != cudaSuccess)
     return e;
   const uint32_t per_cta = ARW2_NT * ARW2_GPT;
   const uint32_t nb = (p->arw2_groups + per_cta - 1) / per_cta;
   const bool sm = p->arw2_ntables == 1; // one table: staged in shared memory
 #define RSB_ARW2(M, S)                                                                     \
-  arw2_kernel<M, S><<<nb, ARW2_NT, 0, st>>>(in, outp, p->d_arw2_jobs, p->nunits,           \
-                                            p->arw2_groups, p->d_arw2_tables, p->d_arw2_bad)
+  arw2_kernel<M, S><<<nb, ARW2_NT, 0, st>>>(in, outp, p->d_arw2_jobs.get(), p->nunits,           \
+                                            p->arw2_groups, p->d_arw2_tables.get(), p->d_job_bad.get())
   if (p->arw2_mode == 0)
     RSB_ARW2(0, false);
   else if (p->arw2_mode == 1) {
@@ -1863,7 +1781,7 @@ static cudaError_t run_sraw_group(const SrawGroup& g, const uint8_t* in, uint8_t
                                   cudaStream_t st) {
   const uint32_t nb = (g.total_mcus + SRAW_NT - 1) / SRAW_NT;
 #define RSB_SRAW(V, T)                                                                     \
-  sraw_kernel<V, T><<<nb, SRAW_NT, 0, st>>>(in, outp, g.d_jobs, g.njobs, g.total_mcus)
+  sraw_kernel<V, T><<<nb, SRAW_NT, 0, st>>>(in, outp, g.d_jobs.get(), g.njobs, g.total_mcus)
   if (g.is420) {
     if (g.version == 1)
       RSB_SRAW(1, true);
@@ -1891,7 +1809,7 @@ static cudaError_t launch_unpack(const UnpackGroup& g, const uint8_t* in, uint64
     attr_set = true;
   }
   unpack_kernel<BPS, LSBO><<<g.nblocks, UNPACK_THREADS, UNPACK_SMEM_BYTES, st>>>(
-      in, in_total, outp, g.d_jobs, g.njobs);
+      in, in_total, outp, g.d_jobs.get(), g.njobs);
   return cudaGetLastError();
 }
 
@@ -1925,7 +1843,7 @@ static cudaError_t launch_unpack_fast(const UnpackFastGroup& g, const uint8_t* i
     attr_set = true;
   }
   unpack_fast_kernel<BPS, LSBO><<<nblocks ? nblocks : g.nblocks, UNPACK_THREADS,
-                                  UNPACK_FAST_SMEM, st>>>(in, outp, g.d_jobs, g.njobs, block_base);
+                                  UNPACK_FAST_SMEM, st>>>(in, outp, g.d_jobs.get(), g.njobs, block_base);
   return cudaGetLastError();
 }
 
@@ -1993,26 +1911,24 @@ static bool par_eligible(const DevScan& d) {
   return thread_eligible(d) && !d.multi_table && d.n_samples >= 8 && d.in_size >= 8;
 }
 
-static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
-                                    const std::vector<DevTable>& ht, ScanBuild& b);
+static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, PlanHolder& plan, const std::vector<DevTable>& ht,
+                                    ScanBuild& b);
 
-static int finish_ljpeg_plan(rsb200_ctx* ctx, rsb200_plan* p,
-                             const rsb200_huff_table* tables, int ntables, ScanBuild& b,
-                             bool /*unused*/) {
+// Lays out and uploads an LJPEG-family plan; on a refusal the caller's holder still owns the plan.
+static int finish_ljpeg_plan(rsb200_ctx* ctx, PlanHolder& plan, const rsb200_huff_table* tables, int ntables,
+                             ScanBuild& b) {
   std::vector<DevTable> ht((size_t)ntables);
   for (int i = 0; i < ntables; ++i)
-    if (!build_dev_table(tables[i], ht[(size_t)i])) {
-      delete p;
+    if (!build_dev_table(tables[i], ht[(size_t)i]))
       return set_err(ctx, RSB200_ERR_ARG, "huffman table %d is malformed", i);
-    }
-  return finish_ljpeg_plan_tables(ctx, p, ht, b);
+  return finish_ljpeg_plan_tables(ctx, plan, ht, b);
 }
 
 // the rest of finish_ljpeg_plan, for plans whose device tables are built by their codec
-static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
-                                    const std::vector<DevTable>& ht, ScanBuild& b) {
+static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, PlanHolder& plan, const std::vector<DevTable>& ht,
+                                    ScanBuild& b) {
+  rsb200_plan* p = plan.get();
   const int ntables = (int)ht.size();
-  p->kind = 1;
   p->ntab_slots = 1;
   for (const DevScan& d : b.scans)
     for (int sl = 0; sl < 4; ++sl)
@@ -2240,22 +2156,11 @@ static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
   p->nranges = (int)ranges.size();
   p->nrows = (uint32_t)b.rows.size();
   cudaError_t e = cudaSuccess;
-  auto up = [&](void** dptr, const void* src, size_t bytes) {
-    if (e != cudaSuccess)
-      return;
-    e = rsb_dev_alloc(dptr, bytes ? bytes : 16);
-    if (e == cudaSuccess && bytes)
-      e = cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice);
-  };
-  auto alloc = [&](void** dptr, size_t bytes) {
-    if (e == cudaSuccess)
-      e = rsb_dev_alloc(dptr, bytes ? bytes : 16);
-  };
-  up((void**)&p->d_tables, ht.data(), sizeof(DevTable) * ht.size());
-  up((void**)&p->d_scans, b.scans.data(), sizeof(DevScan) * b.scans.size());
-  up((void**)&p->d_strips, b.strips.data(), sizeof(DevStrip) * b.strips.size());
-  up((void**)&p->d_rows, b.rows.data(), sizeof(K3RowRef) * b.rows.size());
-  up((void**)&p->d_small_ids, small_ids.data(), sizeof(uint32_t) * small_ids.size());
+  dev_upload(e, p->d_tables, ht.data(), sizeof(DevTable) * ht.size());
+  dev_upload(e, p->d_scans, b.scans.data(), sizeof(DevScan) * b.scans.size());
+  dev_upload(e, p->d_strips, b.strips.data(), sizeof(DevStrip) * b.strips.size());
+  dev_upload(e, p->d_rows, b.rows.data(), sizeof(K3RowRef) * b.rows.size());
+  dev_upload(e, p->d_small_ids, small_ids.data(), sizeof(uint32_t) * small_ids.size());
   {
     // k2_stream_kernel reads "the tile kernel can give this segment a second opinion" from bit 31
     std::vector<uint32_t> ids = thread_ids;
@@ -2263,10 +2168,10 @@ static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
       for (uint32_t& i : ids)
         if (tile_eligible(b.scans[i], TileGeom<1>::MIN_RS))
           i |= 0x80000000u;
-    up((void**)&p->d_thread_ids, ids.data(), sizeof(uint32_t) * ids.size());
+    dev_upload(e, p->d_thread_ids, ids.data(), sizeof(uint32_t) * ids.size());
   }
-  up((void**)&p->d_tile_ids, tile_ids.data(), sizeof(uint32_t) * tile_ids.size());
-  up((void**)&p->d_tile_params, tile_prm.data(), sizeof(DevTileParam) * tile_prm.size());
+  dev_upload(e, p->d_tile_ids, tile_ids.data(), sizeof(uint32_t) * tile_ids.size());
+  dev_upload(e, p->d_tile_params, tile_prm.data(), sizeof(DevTileParam) * tile_prm.size());
   if (!thread_ids.empty()) {
     std::vector<DevTScan> tsc(thread_ids.size());
     uint64_t clean_words = 0, n_anchor = 0;
@@ -2286,7 +2191,7 @@ static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
     if (n_anchor >= (1ull << 32) && !p->use_stream)
       e = cudaErrorInvalidValue;
     if (!p->use_stream)
-      up((void**)&p->d_tscans, tsc.data(), sizeof(DevTScan) * tsc.size());
+      dev_upload(e, p->d_tscans, tsc.data(), sizeof(DevTScan) * tsc.size());
     {
       std::vector<DevTileParam> tp(tsc.size());
       for (size_t k = 0; k < tsc.size(); ++k) {
@@ -2294,36 +2199,32 @@ static int finish_ljpeg_plan_tables(rsb200_ctx* ctx, rsb200_plan* p,
                     tp[k].preroll);
         p->nthread_redo += tsc[k].pad ? 1 : 0;
       }
-      up((void**)&p->d_thread_tile_params, tp.data(), sizeof(DevTileParam) * tp.size());
-      alloc((void**)&p->d_redo, sizeof(uint32_t) * tsc.size());
+      dev_upload(e, p->d_thread_tile_params, tp.data(), sizeof(DevTileParam) * tp.size());
+      dev_alloc(e, p->d_redo, sizeof(uint32_t) * tsc.size());
     }
     if (!p->use_stream) {
-      alloc((void**)&p->d_tinfos, sizeof(DevTInfo) * tsc.size());
-      alloc((void**)&p->d_clean, clean_words * 4 + 256);
-      alloc((void**)&p->d_anchors, n_anchor * 4 + 256);
+      dev_alloc(e, p->d_tinfos, sizeof(DevTInfo) * tsc.size());
+      dev_alloc(e, p->d_clean, clean_words * 4 + 256);
+      dev_alloc(e, p->d_anchors, n_anchor * 4 + 256);
     }
   }
-  up((void**)&p->d_big_ids, big_ids.data(), sizeof(uint32_t) * big_ids.size());
-  up((void**)&p->d_big, big.data(), sizeof(BigScanInfo) * big.size());
-  up((void**)&p->d_ranges, ranges.data(), sizeof(DevRange) * ranges.size());
-  alloc((void**)&p->d_states, sizeof(RangeState) * ranges.size());
-  alloc((void**)&p->d_finals, sizeof(RangeFinal) * ranges.size());
-  alloc((void**)&p->d_fallback, sizeof(uint32_t) * big.size());
-  alloc((void**)&p->d_diffs, (b.diff_elems + 64) * sizeof(uint16_t));
-  alloc((void**)&p->d_colvals, (b.col_elems + 64) * sizeof(uint16_t));
-  alloc((void**)&p->d_results, sizeof(DevResult) * b.scans.size());
-  if (e == cudaSuccess)
-    e = rsb_host_alloc((void**)&p->h_results, sizeof(DevResult) * b.scans.size());
+  dev_upload(e, p->d_big_ids, big_ids.data(), sizeof(uint32_t) * big_ids.size());
+  dev_upload(e, p->d_big, big.data(), sizeof(BigScanInfo) * big.size());
+  dev_upload(e, p->d_ranges, ranges.data(), sizeof(DevRange) * ranges.size());
+  dev_alloc(e, p->d_states, sizeof(RangeState) * ranges.size());
+  dev_alloc(e, p->d_finals, sizeof(RangeFinal) * ranges.size());
+  dev_alloc(e, p->d_fallback, sizeof(uint32_t) * big.size());
+  dev_alloc(e, p->d_diffs, (b.diff_elems + 64) * sizeof(uint16_t));
+  dev_alloc(e, p->d_colvals, (b.col_elems + 64) * sizeof(uint16_t));
+  dev_alloc(e, p->d_results, sizeof(DevResult) * b.scans.size());
+  host_alloc(e, p->h_results, sizeof(DevResult) * b.scans.size());
   if (p->has_pentax) {
-    alloc((void**)&p->d_oob, sizeof(uint32_t) * b.scans.size());
-    if (e == cudaSuccess)
-      e = rsb_host_alloc((void**)&p->h_oob, sizeof(uint32_t) * b.scans.size());
+    dev_alloc(e, p->d_oob, sizeof(uint32_t) * b.scans.size());
+    host_alloc(e, p->h_oob, sizeof(uint32_t) * b.scans.size());
   }
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "ljpeg plan allocation failed: %s",
                    cudaGetErrorString(e));
-  }
   p->launches_per_run = (p->nsmall ? 1 : 0) + (p->ntile ? 1 : 0) + (p->nthread ? (p->use_stream ? 1 : 2) + (p->nthread_redo ? 1 : 0) : 0) +
                         (p->nbig ? 5 + (p->has_k3 ? 2 : 0) + (p->has_pentax ? 2 : 0) + (p->has_nikon ? 2 : 0) : 0);
   return RSB200_OK;
@@ -2338,10 +2239,10 @@ extern "C" int rsb200_pentax_plan_create(rsb200_ctx* ctx, const rsb200_huff_tabl
   if (!ctx || !tables || ntables <= 0 || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "pentax_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   for (int i = 0; i < njobs; ++i) {
     const rsb200_pentax_job& j = jobs[i];
@@ -2350,10 +2251,8 @@ extern "C" int rsb200_pentax_plan_create(rsb200_ctx* ctx, const rsb200_huff_tabl
                     j.height <= 6208 && (int)j.table < ntables && j.in_size < (1u << 28) &&
                     (uint64_t)j.width * 2 <= j.out_pitch && (j.out_offset % 4) == 0 &&
                     (j.out_pitch % 4) == 0;
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "pentax job %d: malformed descriptor", i);
-    }
     DevScan d;
     memset(&d, 0, sizeof d);
     d.in_offset = j.in_offset;
@@ -2383,10 +2282,10 @@ extern "C" int rsb200_pentax_plan_create(rsb200_ctx* ctx, const rsb200_huff_tabl
     p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch + 2ull * j.width));
   }
-  int rc = finish_ljpeg_plan(ctx, p, tables, ntables, b, /*fused=*/false);
+  int rc = finish_ljpeg_plan(ctx, holder, tables, ntables, b);
   if (rc != RSB200_OK)
     return rc;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2423,10 +2322,10 @@ extern "C" int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* j
         (j.out_pitch % 2) || j.reserved0 || j.reserved)
       return set_err(ctx, RSB200_ERR_ARG, "arw1 job %d: malformed descriptor", i);
   }
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   std::vector<DevArw1> fr((size_t)njobs);
   uint64_t koff = 0, runs = 0;
@@ -2483,32 +2382,24 @@ extern "C" int rsb200_arw1_plan_create(rsb200_ctx* ctx, const rsb200_arw1_job* j
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)h - 1) * j.out_pitch + 2ull * w));
   }
   const rsb200_huff_table t = arw1_table();
-  int rc = finish_ljpeg_plan(ctx, p, &t, 1, b, /*fused=*/false);
+  int rc = finish_ljpeg_plan(ctx, holder, &t, 1, b);
   if (rc != RSB200_OK)
     return rc;
   for (size_t i = 0; i < fr.size(); ++i)
     fr[i].diff_offset = b.scans[i].diff_offset;
   p->narw1 = njobs;
   p->arw1_in_bytes = koff;
-  cudaError_t e = rsb_dev_alloc((void**)&p->d_arw1, sizeof(DevArw1) * fr.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_arw1, fr.data(), sizeof(DevArw1) * fr.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw1_in, koff + 256);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw1_runs, sizeof(Arw1Run) * runs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw1_lastoff, sizeof(uint32_t) * runs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw1_runpre, sizeof(int2) * runs);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_arw1_info, sizeof(Arw1Info) * fr.size());
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_arw1, fr.data(), sizeof(DevArw1) * fr.size());
+  dev_alloc(e, p->d_arw1_in, koff + 256);
+  dev_alloc(e, p->d_arw1_runs, sizeof(Arw1Run) * runs);
+  dev_alloc(e, p->d_arw1_lastoff, sizeof(uint32_t) * runs);
+  dev_alloc(e, p->d_arw1_runpre, sizeof(int2) * runs);
+  dev_alloc(e, p->d_arw1_info, sizeof(Arw1Info) * fr.size());
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "arw1 plan allocation failed: %s", cudaGetErrorString(e));
-  }
   p->launches_per_run += 4;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2534,10 +2425,10 @@ extern "C" int rsb200_samsung1_plan_create(rsb200_ctx* ctx, const rsb200_samsung
         (j.out_pitch % 4) || j.reserved)
       return set_err(ctx, RSB200_ERR_ARG, "samsung1 job %d: malformed descriptor", i);
   }
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   std::vector<DevS1> fr((size_t)njobs);
   uint64_t rows = 0;
@@ -2584,35 +2475,26 @@ extern "C" int rsb200_samsung1_plan_create(rsb200_ctx* ctx, const rsb200_samsung
   }
   // (the row kernels' 1-D grids: one CTA per 8 rows of the tallest frame, per frame)
   if (rows >= (1ull << 31) ||
-      (uint64_t)njobs * ((p->s1_max_h + S1_ROWS_PER_CTA - 1) / S1_ROWS_PER_CTA) >= (1ull << 31)) {
-    delete p;
+      (uint64_t)njobs * ((p->s1_max_h + S1_ROWS_PER_CTA - 1) / S1_ROWS_PER_CTA) >= (1ull << 31))
     return set_err(ctx, RSB200_ERR_ARG, "samsung1 plan: too many frames for one plan");
-  }
   std::vector<DevTable> ht(1);
   samsung1_dev_table(ht[0]);
-  int rc = finish_ljpeg_plan_tables(ctx, p, ht, b);
+  int rc = finish_ljpeg_plan_tables(ctx, holder, ht, b);
   if (rc != RSB200_OK)
     return rc;
   for (size_t i = 0; i < fr.size(); ++i)
     fr[i].diff_offset = b.scans[i].diff_offset;
   p->ns1 = njobs;
-  cudaError_t e = rsb_dev_alloc((void**)&p->d_s1, sizeof(DevS1) * fr.size());
-  if (e == cudaSuccess)
-    e = cudaMemcpy(p->d_s1, fr.data(), sizeof(DevS1) * fr.size(), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_s1_colvals, sizeof(uint16_t) * 2 * rows);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_s1_rowbits, sizeof(uint2) * rows);
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_s1_oob, sizeof(uint32_t) * fr.size());
-  if (e == cudaSuccess)
-    e = rsb_dev_alloc((void**)&p->d_s1_lim, sizeof(uint32_t) * fr.size());
-  if (e != cudaSuccess) {
-    rsb200_plan_destroy(p);
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_s1, fr.data(), sizeof(DevS1) * fr.size());
+  dev_alloc(e, p->d_s1_colvals, sizeof(uint16_t) * 2 * rows);
+  dev_alloc(e, p->d_s1_rowbits, sizeof(uint2) * rows);
+  dev_alloc(e, p->d_s1_oob, sizeof(uint32_t) * fr.size());
+  dev_alloc(e, p->d_s1_lim, sizeof(uint32_t) * fr.size());
+  if (e != cudaSuccess)
     return set_err(ctx, RSB200_ERR_CUDA, "samsung1 plan allocation failed: %s", cudaGetErrorString(e));
-  }
   p->launches_per_run += 4;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2626,10 +2508,10 @@ extern "C" int rsb200_nikon_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
       nluts > 254 || (nluts > 0 && !luts))
     return set_err(ctx, RSB200_ERR_ARG, "nikon_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   for (int i = 0; i < njobs; ++i) {
     const rsb200_nikon_job& j = jobs[i];
@@ -2638,10 +2520,8 @@ extern "C" int rsb200_nikon_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
                     j.height <= 5520 && (int)j.table < ntables && j.in_size >= 4 &&
                     j.in_size < (1u << 28) && (uint64_t)j.width * 2 <= j.out_pitch &&
                     (j.out_offset % 4) == 0 && (j.out_pitch % 4) == 0 && j.lut < nluts;
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "nikon job %d: malformed descriptor", i);
-    }
     DevScan d;
     memset(&d, 0, sizeof d);
     d.in_offset = j.in_offset;
@@ -2674,20 +2554,14 @@ extern "C" int rsb200_nikon_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
     p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch + 2ull * j.width));
   }
-  int rc = finish_ljpeg_plan(ctx, p, tables, ntables, b, /*fused=*/false);
+  int rc = finish_ljpeg_plan(ctx, holder, tables, ntables, b);
   if (rc != RSB200_OK)
     return rc;
-  {
-    const size_t bytes = (size_t)nluts * 2u * 65536u * sizeof(uint16_t);
-    cudaError_t e = rsb_dev_alloc((void**)&p->d_nikon_luts, bytes + 16);
-    if (e == cudaSuccess && bytes)
-      e = cudaMemcpy(p->d_nikon_luts, luts, bytes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      rsb200_plan_destroy(p);
-      return set_err(ctx, RSB200_ERR_CUDA, "nikon plan upload failed: %s", cudaGetErrorString(e));
-    }
-  }
-  *out = p;
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, p->d_nikon_luts, luts, (size_t)nluts * 2u * 65536u * sizeof(uint16_t), 16);
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "nikon plan upload failed: %s", cudaGetErrorString(e));
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2697,10 +2571,10 @@ extern "C" int rsb200_ljpeg_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
   if (!ctx || !tables || ntables <= 0 || !scans || nscans <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "ljpeg_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   b.scans.reserve((size_t)nscans);
   for (int i = 0; i < nscans; ++i) {
@@ -2708,10 +2582,8 @@ extern "C" int rsb200_ljpeg_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
     const int group = s.mcu_w * s.mcu_h;
     DevScan d;
     // validation (every sum in 64 bits, out_offset 2-byte aligned) + descriptor: ljpeg_host.h
-    if (!ljpeg_scan_to_dev(s, ntables, d)) {
-      delete p;
+    if (!ljpeg_scan_to_dev(s, ntables, d))
       return set_err(ctx, RSB200_ERR_ARG, "ljpeg scan %d: malformed descriptor", i);
-    }
     (void)group;
     d.diff_offset = b.diff_elems;
     b.diff_elems += ((uint64_t)d.n_samples + 7) & ~7ull;
@@ -2727,16 +2599,14 @@ extern "C" int rsb200_ljpeg_plan_create(rsb200_ctx* ctx, const rsb200_huff_table
     p->need_in = std::max<uint64_t>(p->need_in, sat_add(s.in_offset, s.in_size));
     const uint64_t last_row = (uint64_t)s.out_y + (uint64_t)s.rows * s.mcu_h - 1;
     const uint64_t extent = last_row * s.out_pitch + 2ull * ((uint64_t)s.out_x + s.store_w);
-    if (s.out_offset + extent < s.out_offset || s.in_offset + (uint64_t)s.in_size < s.in_offset) {
-      delete p;
+    if (s.out_offset + extent < s.out_offset || s.in_offset + (uint64_t)s.in_size < s.in_offset)
       return set_err(ctx, RSB200_ERR_ARG, "ljpeg scan %d: offset + extent overflows", i);
-    }
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(s.out_offset, extent));
   }
-  int rc = finish_ljpeg_plan(ctx, p, tables, ntables, b, /*fused=*/true);
+  int rc = finish_ljpeg_plan(ctx, holder, tables, ntables, b);
   if (rc != RSB200_OK)
     return rc;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2786,10 +2656,10 @@ extern "C" int rsb200_cr2_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* 
   if (!ctx || !tables || ntables <= 0 || !jobs || njobs <= 0 || !out)
     return set_err(ctx, RSB200_ERR_ARG, "cr2_plan_create: bad arguments");
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
-  rsb200_plan* p = new (std::nothrow) rsb200_plan();
-  if (!p)
+  PlanHolder holder = new_plan(ctx, PlanKind::Ljpeg);
+  if (!holder)
     return RSB200_ERR_CUDA;
-  p->ctx = ctx;
+  rsb200_plan* p = holder.get();
   ScanBuild b;
   for (int i = 0; i < njobs; ++i) {
     const rsb200_cr2_job& j = jobs[i];
@@ -2826,10 +2696,8 @@ extern "C" int rsb200_cr2_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* 
       d.n_samples = (uint32_t)(total_groups * groupSize);
       ok = ok && total_groups * groupSize < (1ull << 32);
     }
-    if (!ok) {
-      delete p;
+    if (!ok)
       return set_err(ctx, RSB200_ERR_ARG, "cr2 job %d: malformed descriptor", i);
-    }
     d.in_offset = j.in_offset;
     d.in_size = j.in_size;
     d.group = (uint8_t)groupSize;
@@ -2863,10 +2731,10 @@ extern "C" int rsb200_cr2_plan_create(rsb200_ctx* ctx, const rsb200_huff_table* 
     p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
     p->need_out = std::max<uint64_t>(p->need_out, sat_add(j.out_offset, ((uint64_t)j.img_h - 1) * j.out_pitch + 2ull * j.img_w));
   }
-  int rc = finish_ljpeg_plan(ctx, p, tables, ntables, b, /*fused=*/false);
+  int rc = finish_ljpeg_plan(ctx, holder, tables, ntables, b);
   if (rc != RSB200_OK)
     return rc;
-  *out = p;
+  *out = holder.release();
   return RSB200_OK;
 }
 
@@ -2911,7 +2779,8 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
   cudaStream_t st = (cudaStream_t)stream;
   const uint8_t* in = (const uint8_t*)d_in;
   uint8_t* outp = (uint8_t*)d_out;
-  if (p->kind == 0) {
+  switch (p->kind) {
+  case PlanKind::Unpack:
     for (const UnpackFastGroup& g : p->fast_groups) {
       if (!g.nblocks)
         continue;
@@ -2924,99 +2793,113 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
       CUDA_TRY(ctx, run_unpack_group(g, in, (uint64_t)in_bytes, outp, st));
       ctx->launches++;
     }
-  } else if (p->kind == 10) {
+    break;
+  case PlanKind::Lookup: {
     const uint32_t nbs = (uint32_t)(((uint64_t)p->lookup_quads * p->lookup_nseg + LUT_WARPS - 1) / LUT_WARPS);
     if (p->lookup_smem && !p->lookup_dither && p->lookup_ntables == 1) {
       const int sms = ctx->sm_count;
       lookup_smem_kernel<<<(unsigned)std::max(1, sms), LUT_SMEM_NT, LUT_SMEM_BYTES, st>>>(
-          outp, p->d_lookup_jobs, p->lookup_njobs, p->lookup_quads, p->d_lookup_tables);
+          outp, p->d_lookup_jobs.get(), p->lookup_njobs, p->lookup_quads, p->d_lookup_tables.get());
     } else if (p->lookup_dither)
-      lookup_kernel<true><<<nbs, LUT_NT, 0, st>>>(outp, p->d_lookup_jobs, p->lookup_njobs, p->lookup_quads,
-                                                  p->d_lookup_tables, p->lookup_nseg);
+      lookup_kernel<true><<<nbs, LUT_NT, 0, st>>>(outp, p->d_lookup_jobs.get(), p->lookup_njobs, p->lookup_quads,
+                                                  p->d_lookup_tables.get(), p->lookup_nseg);
     else
-      lookup_kernel<false><<<nbs, LUT_NT, 0, st>>>(outp, p->d_lookup_jobs, p->lookup_njobs, p->lookup_quads,
-                                                   p->d_lookup_tables, p->lookup_nseg);
+      lookup_kernel<false><<<nbs, LUT_NT, 0, st>>>(outp, p->d_lookup_jobs.get(), p->lookup_njobs, p->lookup_quads,
+                                                   p->d_lookup_tables.get(), p->lookup_nseg);
     CUDA_TRY(ctx, cudaGetLastError());
     ctx->launches++;
-  } else if (p->kind == 9) {
+    break;
+  }
+  case PlanKind::BadPix:
     if (p->badpix_total) {
       badpix_kernel<<<(p->badpix_total + BADPIX_NT - 1) / BADPIX_NT, BADPIX_NT, 0, st>>>(
-          outp, p->d_badpix_jobs, p->badpix_njobs, p->d_badpix_list, p->badpix_total, p->d_badpix_maps);
+          outp, p->d_badpix_jobs.get(), p->badpix_njobs, p->d_badpix_list.get(), p->badpix_total, p->d_badpix_maps.get());
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches++;
     }
-  } else if (p->kind == 8) {
-    if (p->pana_zero_slots)
-      CUDA_TRY(ctx, cudaMemsetAsync(p->d_pana_zero_count, 0,
-                                    sizeof(uint32_t) * (size_t)p->pana_zero_slots, st));
+    break;
+  case PlanKind::DngOp:
+    if (p->nbad_slots)
+      CUDA_TRY(ctx, cudaMemsetAsync(p->d_bad_count.get(), 0,
+                                    sizeof(uint32_t) * (size_t)p->nbad_slots, st));
     if (p->dngop_units) {
       dngop_kernel<<<(p->dngop_units + DNGOP_NT - 1) / DNGOP_NT, DNGOP_NT, 0, st>>>(
-          outp, p->d_dngop_jobs, p->dngop_njobs, p->dngop_units, p->d_dngop_ops, p->d_dngop_tables,
-          p->d_dngop_deltas, p->d_pana_zero_count, p->d_pana_zero_list);
+          outp, p->d_dngop_jobs.get(), p->dngop_njobs, p->dngop_units, p->d_dngop_ops.get(), p->d_dngop_tables.get(),
+          p->d_dngop_deltas.get(), p->d_bad_count.get(), p->d_bad_list.get());
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches++;
     }
-  } else if (p->kind == 7) {
+    break;
+  case PlanKind::Scale:
     for (const ScaleGroup& g : p->scale_groups) {
       const uint32_t nb = (g.total_quads + SCALE_WARPS - 1) / SCALE_WARPS;
       if (g.mode == 0)
-        scale_kernel<0><<<nb, SCALE_NT, 0, st>>>(outp, g.d_jobs, g.njobs, g.total_quads, 1u);
+        scale_kernel<0><<<nb, SCALE_NT, 0, st>>>(outp, g.d_jobs.get(), g.njobs, g.total_quads, 1u);
       else
         scale_kernel<1><<<(uint32_t)(((uint64_t)g.total_quads * g.nseg + SCALE_WARPS - 1) / SCALE_WARPS), SCALE_NT,
-                          0, st>>>(outp, g.d_jobs, g.njobs, g.total_quads, g.nseg);
+                          0, st>>>(outp, g.d_jobs.get(), g.njobs, g.total_quads, g.nseg);
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches++;
     }
-  } else if (p->kind == 11) {
+    break;
+  case PlanKind::Hasselblad:
     CUDA_TRY(ctx, run_hasselblad(p, in, outp, st));
     ctx->launches += (uint64_t)p->launches_per_run;
-  } else if (p->kind == 6) {
+    break;
+  case PlanKind::PhaseOne:
     CUDA_TRY(ctx, run_phaseone(p, in, outp, st));
-    ctx->launches++;
-  } else if (p->kind == 12) {
+    ctx->launches += (uint64_t)p->launches_per_run;
+    break;
+  case PlanKind::SamsungV0:
     CUDA_TRY(ctx, run_samsung0(p, in, outp, st));
     ctx->launches += (uint64_t)p->launches_per_run;
-  } else if (p->kind == 13) {
+    break;
+  case PlanKind::SamsungV2:
     CUDA_TRY(ctx, run_samsung2(p, in, outp, st));
     ctx->launches += (uint64_t)p->launches_per_run;
-  } else if (p->kind == 5) {
+    break;
+  case PlanKind::Pana:
     for (const PanaGroup& g : p->pana_groups) {
       CUDA_TRY(ctx, run_pana_group(p, g, in, outp, st));
       ctx->launches++;
     }
-  } else if (p->kind == 4) {
+    break;
+  case PlanKind::Arw2:
     CUDA_TRY(ctx, run_arw2(p, in, outp, st));
     ctx->launches++;
-  } else if (p->kind == 3) {
+    break;
+  case PlanKind::Sraw:
     for (const SrawGroup& g : p->sraw_groups) {
       CUDA_TRY(ctx, run_sraw_group(g, in, outp, st));
       ctx->launches++;
     }
-  } else if (p->kind == 2) {
+    break;
+  case PlanKind::RawForm:
     for (const RawGroup& g : p->raw_groups) {
       if (!g.total_items)
         continue;
-      CUDA_TRY(ctx, run_raw_group(g, in, (uint64_t)in_bytes, outp, p->d_raw_tables, st));
+      CUDA_TRY(ctx, run_raw_group(g, in, (uint64_t)in_bytes, outp, p->d_raw_tables.get(), st));
       ctx->launches++;
     }
-  } else {
+    break;
+  case PlanKind::Ljpeg: {
     const size_t fsm = fused_smem_bytes(p->ntab_slots);
     if (p->ntile) {
       if (p->tile_r == 2)
         k2_tile_kernel<2><<<p->ntile, TL_NT, tile_smem_bytes<2>(), st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, outp, p->d_results, p->d_tile_ids,
-            p->d_tile_params, nullptr);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), outp, p->d_results.get(), p->d_tile_ids.get(),
+            p->d_tile_params.get(), nullptr);
       else
         k2_tile_kernel<1><<<p->ntile, TL_NT, tile_smem_bytes<1>(), st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, outp, p->d_results, p->d_tile_ids,
-            p->d_tile_params, nullptr);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), outp, p->d_results.get(), p->d_tile_ids.get(),
+            p->d_tile_params.get(), nullptr);
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 1;
     }
     if (p->nsmall) {
-      k2_fused_kernel<<<p->nsmall, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans,
-                                                     p->d_tables, outp, p->d_results,
-                                                     p->d_small_ids);
+      k2_fused_kernel<<<p->nsmall, F_NT, fsm, st>>>(in, (uint64_t)in_bytes, p->d_scans.get(),
+                                                     p->d_tables.get(), outp, p->d_results.get(),
+                                                     p->d_small_ids.get());
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 1;
     }
@@ -3028,25 +2911,25 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
       const size_t smem = stream_smem_bytes(p->ntables);
       if (!stream_full_launch(ctx, p))
         k2_stream_kernel<false, false><<<nb, T_NT, smem, st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
-            p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 1);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), p->ntables, outp, p->d_results.get(),
+            p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_redo.get(), 1);
       else if (stream_staged(p->ntables))
         k2_stream_kernel<true, true><<<nb, T_NT, smem, st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
-            p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 0);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), p->ntables, outp, p->d_results.get(),
+            p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_redo.get(), 0);
       else
         k2_stream_kernel<true, false><<<nb, T_NT, smem, st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, p->ntables, outp, p->d_results,
-            p->d_thread_ids, (uint32_t)p->nthread, p->d_redo, 0);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), p->ntables, outp, p->d_results.get(),
+            p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_redo.get(), 0);
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 1;
     } else if (p->nthread && p->use_par) {
       k2_clean_kernel<<<(p->nthread + C_WARPS - 1) / C_WARPS, 32 * C_WARPS, 0, st>>>(
-          in, (uint64_t)in_bytes, p->d_scans, p->d_thread_ids, (uint32_t)p->nthread, p->d_tscans,
-          p->d_clean, p->d_anchors, p->d_tinfos);
+          in, (uint64_t)in_bytes, p->d_scans.get(), p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_tscans.get(),
+          p->d_clean.get(), p->d_anchors.get(), p->d_tinfos.get());
       k2_par_kernel<<<p->par_ctas > 0 ? std::min(p->nthread, ctx->sm_count * p->par_ctas) : p->nthread, P_NT, 0, st>>>(
-          in, p->d_scans, p->d_tables, outp, p->d_results, p->d_thread_ids, (uint32_t)p->nthread, p->d_tscans,
-          p->d_tinfos, p->d_clean, p->d_anchors, p->d_diffs, p->d_redo);
+          in, p->d_scans.get(), p->d_tables.get(), outp, p->d_results.get(), p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_tscans.get(),
+          p->d_tinfos.get(), p->d_clean.get(), p->d_anchors.get(), p->d_diffs.get(), p->d_redo.get());
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 2;
     } else if (p->nthread) {
@@ -3054,15 +2937,15 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
       // segments (k2_clean2_kernel), one warp per segment for small ones (k2_clean_kernel)
       if (p->clean2)
         k2_clean2_kernel<<<p->nthread, TL_NT, tile_smem_bytes<1>(), st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_thread_ids, (uint32_t)p->nthread, p->d_tscans,
-            p->d_clean, p->d_anchors, p->d_tinfos);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_tscans.get(),
+            p->d_clean.get(), p->d_anchors.get(), p->d_tinfos.get());
       else
       k2_clean_kernel<<<(p->nthread + C_WARPS - 1) / C_WARPS, 32 * C_WARPS, 0, st>>>(
-          in, (uint64_t)in_bytes, p->d_scans, p->d_thread_ids, (uint32_t)p->nthread, p->d_tscans,
-          p->d_clean, p->d_anchors, p->d_tinfos);
+          in, (uint64_t)in_bytes, p->d_scans.get(), p->d_thread_ids.get(), (uint32_t)p->nthread, p->d_tscans.get(),
+          p->d_clean.get(), p->d_anchors.get(), p->d_tinfos.get());
       k2_thread_kernel<<<(p->nthread + T_NT - 1) / T_NT, T_NT, thread_smem_bytes(p->ntables), st>>>(
-          in, p->d_scans, p->d_tables, p->ntables, outp, p->d_results, p->d_thread_ids,
-          (uint32_t)p->nthread, p->d_tscans, p->d_tinfos, p->d_clean, p->d_anchors, p->d_redo);
+          in, p->d_scans.get(), p->d_tables.get(), p->ntables, outp, p->d_results.get(), p->d_thread_ids.get(),
+          (uint32_t)p->nthread, p->d_tscans.get(), p->d_tinfos.get(), p->d_clean.get(), p->d_anchors.get(), p->d_redo.get());
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 2;
     }
@@ -3070,87 +2953,89 @@ extern "C" int rsb200_plan_run(rsb200_plan* p, const void* d_in, size_t in_bytes
       if (p->nthread_redo) {
         // exact end-of-stream semantics for the segments K2T flagged (CTAs of the others exit at once)
         k2_tile_kernel<1><<<p->nthread, TL_NT, tile_smem_bytes<1>(), st>>>(
-            in, (uint64_t)in_bytes, p->d_scans, p->d_tables, outp, p->d_results, p->d_thread_ids,
-            p->d_thread_tile_params, p->d_redo);
+            in, (uint64_t)in_bytes, p->d_scans.get(), p->d_tables.get(), outp, p->d_results.get(), p->d_thread_ids.get(),
+            p->d_thread_tile_params.get(), p->d_redo.get());
         CUDA_TRY(ctx, cudaGetLastError());
         ctx->launches += 1;
       }
     }
     if (p->nbig) {
-      k2_clear_results_kernel<<<(p->nbig + 127) / 128, 128, 0, st>>>(p->d_big, p->nbig,
-                                                                     p->d_results, p->d_oob);
+      k2_clear_results_kernel<<<(p->nbig + 127) / 128, 128, 0, st>>>(p->d_big.get(), p->nbig,
+                                                                     p->d_results.get(), p->d_oob.get());
       // ARW1 frames: the range decoder reads the complemented copies (arw1.cuh)
       const uint8_t* kin = in;
       uint64_t kin_bytes = (uint64_t)in_bytes;
       if (p->has_arw1) {
         arw1_prep_kernel<<<dim3((p->arw1_max_words + 255) / 256, p->narw1), 256, 0, st>>>(
-            in, p->d_arw1_in, p->d_arw1);
-        kin = p->d_arw1_in;
+            in, p->d_arw1_in.get(), p->d_arw1.get());
+        kin = p->d_arw1_in.get();
         kin_bytes = p->arw1_in_bytes;
       }
-      k2_range_count_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans,
-                                                           p->d_tables, p->d_ranges, p->d_states);
-      k2_range_verify_kernel<<<p->nbig, V_NT, 0, st>>>(p->d_scans, p->d_big, p->d_states,
-                                                       p->d_finals, p->d_fallback, p->d_results);
-      k2_range_diffs_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans,
-                                                           p->d_tables, p->d_ranges, p->d_finals,
-                                                           p->d_diffs, p->d_results);
+      k2_range_count_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans.get(),
+                                                           p->d_tables.get(), p->d_ranges.get(), p->d_states.get());
+      k2_range_verify_kernel<<<p->nbig, V_NT, 0, st>>>(p->d_scans.get(), p->d_big.get(), p->d_states.get(),
+                                                       p->d_finals.get(), p->d_fallback.get(), p->d_results.get());
+      k2_range_diffs_kernel<<<p->nranges, F_NT, fsm, st>>>(kin, kin_bytes, p->d_scans.get(),
+                                                           p->d_tables.get(), p->d_ranges.get(), p->d_finals.get(),
+                                                           p->d_diffs.get(), p->d_results.get());
       // exact redo of segments whose speculative parse failed verification (no-op otherwise)
       k2_entropy_kernel<<<p->nbig, K2_THREADS, sizeof(K2Shared), st>>>(
-          kin, kin_bytes, p->d_scans, p->d_tables, p->d_diffs, p->d_results,
-          p->d_big_ids, p->d_fallback);
+          kin, kin_bytes, p->d_scans.get(), p->d_tables.get(), p->d_diffs.get(), p->d_results.get(),
+          p->d_big_ids.get(), p->d_fallback.get());
       const int col_warps = p->nbig * 4;
       const uint32_t rows_per_block = K3_THREADS / 32;
       int nk3 = 0;
       if (p->has_k3) {
         k3_column_kernel<<<(col_warps * 32 + 127) / 128, 128, 0, st>>>(
-            p->d_scans, p->d_big_ids, p->nbig, p->d_diffs, p->d_colvals);
+            p->d_scans.get(), p->d_big_ids.get(), p->nbig, p->d_diffs.get(), p->d_colvals.get());
         k3_row_kernel<<<(p->nrows + rows_per_block - 1) / rows_per_block, K3_THREADS, 0, st>>>(
-            p->d_scans, p->d_rows, p->nrows, p->d_diffs, p->d_colvals, p->d_strips, outp);
+            p->d_scans.get(), p->d_rows.get(), p->nrows, p->d_diffs.get(), p->d_colvals.get(), p->d_strips.get(), outp);
         nk3 += 2;
       }
       if (p->has_pentax) {
         k3p_column_kernel<<<(col_warps * 32 + 127) / 128, 128, 0, st>>>(
-            p->d_scans, p->d_big_ids, p->nbig, p->d_diffs, p->d_colvals, p->d_oob);
+            p->d_scans.get(), p->d_big_ids.get(), p->nbig, p->d_diffs.get(), p->d_colvals.get(), p->d_oob.get());
         k3p_row_kernel<<<(p->nrows + rows_per_block - 1) / rows_per_block, K3_THREADS, 0, st>>>(
-            p->d_scans, p->d_rows, p->nrows, p->d_diffs, p->d_colvals, outp, p->d_oob);
+            p->d_scans.get(), p->d_rows.get(), p->nrows, p->d_diffs.get(), p->d_colvals.get(), outp, p->d_oob.get());
         nk3 += 2;
       }
       if (p->has_nikon) {
         k3n_column_kernel<<<(col_warps * 32 + 127) / 128, 128, 0, st>>>(
-            p->d_scans, p->d_big_ids, p->nbig, p->d_diffs, p->d_colvals);
+            p->d_scans.get(), p->d_big_ids.get(), p->nbig, p->d_diffs.get(), p->d_colvals.get());
         k3n_row_kernel<<<(p->nrows + rows_per_block - 1) / rows_per_block, K3_THREADS, 0, st>>>(
-            in, p->d_scans, p->d_rows, p->nrows, p->d_diffs, p->d_colvals, p->d_nikon_luts, outp);
+            in, p->d_scans.get(), p->d_rows.get(), p->nrows, p->d_diffs.get(), p->d_colvals.get(), p->d_nikon_luts.get(), outp);
         nk3 += 2;
       }
       if (p->has_arw1) {
         arw1_runsum_kernel<<<dim3((p->arw1_max_runs + ARW1_NT / 32 - 1) / (ARW1_NT / 32), p->narw1),
-                             ARW1_NT, 0, st>>>(p->d_arw1, p->d_diffs, p->d_arw1_runs,
-                                               p->d_arw1_lastoff);
-        arw1_scan_kernel<<<p->narw1, ARW1_SCAN_NT, 0, st>>>(p->d_arw1, p->d_arw1_runs,
-                                                            p->d_arw1_lastoff, p->d_arw1_runpre,
-                                                            p->d_arw1_info, p->d_results);
+                             ARW1_NT, 0, st>>>(p->d_arw1.get(), p->d_diffs.get(), p->d_arw1_runs.get(),
+                                               p->d_arw1_lastoff.get());
+        arw1_scan_kernel<<<p->narw1, ARW1_SCAN_NT, 0, st>>>(p->d_arw1.get(), p->d_arw1_runs.get(),
+                                                            p->d_arw1_lastoff.get(), p->d_arw1_runpre.get(),
+                                                            p->d_arw1_info.get(), p->d_results.get());
         arw1_apply_kernel<<<dim3(p->arw1_max_tiles, p->narw1), ARW1_NT, 0, st>>>(
-            p->d_arw1, p->d_diffs, p->d_arw1_runpre, p->d_arw1_info, outp, p->d_results);
+            p->d_arw1.get(), p->d_diffs.get(), p->d_arw1_runpre.get(), p->d_arw1_info.get(), outp, p->d_results.get());
         nk3 += 4;
       }
       if (p->has_samsung1) {
-        CUDA_TRY(ctx, cudaMemsetAsync(p->d_s1_oob, 0xFF, sizeof(uint32_t) * (size_t)p->ns1, st));
+        CUDA_TRY(ctx, cudaMemsetAsync(p->d_s1_oob.get(), 0xFF, sizeof(uint32_t) * (size_t)p->ns1, st));
         const uint32_t rb = (p->s1_max_h + S1_ROWS_PER_CTA - 1) / S1_ROWS_PER_CTA;
         const uint32_t rows_grid = rb * (uint32_t)p->ns1; // (< 2^31: checked at plan creation)
-        s1_column_kernel<<<(p->ns1 * 4 * 32 + 127) / 128, 128, 0, st>>>(p->d_s1, p->ns1, p->d_diffs,
-                                                                        p->d_s1_colvals, p->d_s1_oob);
-        s1_row_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1, rb, p->d_diffs, p->d_s1_colvals,
-                                                   p->d_s1_rowbits, p->d_s1_oob);
-        s1_scan_kernel<<<p->ns1, S1_SCAN_NT, 0, st>>>(p->d_s1, p->d_diffs, p->d_s1_rowbits,
-                                                      p->d_s1_oob, p->d_s1_lim, p->d_results);
-        s1_store_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1, rb, p->d_diffs, p->d_s1_colvals,
-                                                     p->d_s1_lim, outp);
+        s1_column_kernel<<<(p->ns1 * 4 * 32 + 127) / 128, 128, 0, st>>>(p->d_s1.get(), p->ns1, p->d_diffs.get(),
+                                                                        p->d_s1_colvals.get(), p->d_s1_oob.get());
+        s1_row_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1.get(), rb, p->d_diffs.get(), p->d_s1_colvals.get(),
+                                                   p->d_s1_rowbits.get(), p->d_s1_oob.get());
+        s1_scan_kernel<<<p->ns1, S1_SCAN_NT, 0, st>>>(p->d_s1.get(), p->d_diffs.get(), p->d_s1_rowbits.get(),
+                                                      p->d_s1_oob.get(), p->d_s1_lim.get(), p->d_results.get());
+        s1_store_kernel<<<rows_grid, S1_NT, 0, st>>>(p->d_s1.get(), rb, p->d_diffs.get(), p->d_s1_colvals.get(),
+                                                     p->d_s1_lim.get(), outp);
         nk3 += 4;
       }
       CUDA_TRY(ctx, cudaGetLastError());
       ctx->launches += 5 + nk3;
     }
+    break;
+  }
   }
   p->last_stream = st;
   p->ran = true;
@@ -3175,7 +3060,7 @@ static int ensure_cap(rsb200_ctx* ctx, uint8_t** buf, size_t* cap, size_t need) 
 // upload of the next frame and the download of the previous one overlap the
 // unpack of the current one (both PCIe directions busy).
 static bool unpack_pipeline_ok(const rsb200_plan* p) {
-  if (p->kind != 0 || !p->groups.empty() || p->fast_groups.size() != 1)
+  if (p->kind != PlanKind::Unpack || !p->groups.empty() || p->fast_groups.size() != 1)
     return false;
   const auto& jobs = p->fast_groups[0].h_jobs;
   if (jobs.size() < 2)
@@ -3280,12 +3165,12 @@ static cudaError_t launch_tile_range(const rsb200_plan* p, const uint8_t* d_in, 
                                      cudaStream_t st) {
   if (p->tile_r == 2)
     k2_tile_kernel<2><<<count, TL_NT, tile_smem_bytes<2>(), st>>>(
-        d_in, in_bytes, p->d_scans, p->d_tables, d_out, p->d_results, p->d_tile_ids + first,
-        p->d_tile_params + first, nullptr);
+        d_in, in_bytes, p->d_scans.get(), p->d_tables.get(), d_out, p->d_results.get(), p->d_tile_ids.get() + first,
+        p->d_tile_params.get() + first, nullptr);
   else
     k2_tile_kernel<1><<<count, TL_NT, tile_smem_bytes<1>(), st>>>(
-        d_in, in_bytes, p->d_scans, p->d_tables, d_out, p->d_results, p->d_tile_ids + first,
-        p->d_tile_params + first, nullptr);
+        d_in, in_bytes, p->d_scans.get(), p->d_tables.get(), d_out, p->d_results.get(), p->d_tile_ids.get() + first,
+        p->d_tile_params.get() + first, nullptr);
   return cudaGetLastError();
 }
 
@@ -3422,11 +3307,11 @@ extern "C" int rsb200_plan_run_host(rsb200_plan* p, const uint8_t* in, size_t in
     return rc;
   if (in_bytes < p->need_in || out_bytes < p->need_out)
     return set_err(ctx, RSB200_ERR_ARG, "plan_run_host: buffers too small");
-  if (p->kind >= 7 && p->kind <= 10)
+  if (in_place(p->kind))
     partial = 1; // in-place plans work on the image the caller holds: it always goes up first
   if (!partial && unpack_pipeline_ok(p))
     return run_host_unpack_pipelined(p, in, in_bytes, out, out_bytes);
-  if (!partial && p->kind == 1 && p->tile_groups.size() >= 2 && !getenv("RSB200_NO_PIPELINE"))
+  if (!partial && p->kind == PlanKind::Ljpeg && p->tile_groups.size() >= 2 && !getenv("RSB200_NO_PIPELINE"))
     return run_host_tile_pipelined(p, in, in_bytes, out, out_bytes);
   cudaStream_t st = ctx->stream;
   const bool stage_in = in_bytes && in_bytes <= STAGE_LIMIT && host_is_pageable(in);
@@ -3472,7 +3357,7 @@ extern "C" int rsb200_plan_run_host_image(rsb200_plan* p, const uint8_t* in, siz
   rsb200_ctx* ctx = p->ctx;
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   const size_t out_bytes = (size_t)pitch * rows;
-  if (p->kind >= 7 && p->kind <= 10)
+  if (in_place(p->kind))
     partial = 1; // in-place plans: the image always goes up first
   int rc = ensure_cap(ctx, &ctx->d_in, &ctx->d_in_cap, in_bytes + 16);
   if (rc)
@@ -3482,7 +3367,7 @@ extern "C" int rsb200_plan_run_host_image(rsb200_plan* p, const uint8_t* in, siz
     return rc;
   if (in_bytes < p->need_in || out_bytes < p->need_out)
     return set_err(ctx, RSB200_ERR_ARG, "plan_run_host_image: buffers too small");
-  if (!partial && p->kind == 1 && p->tile_groups.size() >= 2 && !getenv("RSB200_NO_PIPELINE"))
+  if (!partial && p->kind == PlanKind::Ljpeg && p->tile_groups.size() >= 2 && !getenv("RSB200_NO_PIPELINE"))
     return run_host_tile_pipelined(p, in, in_bytes, out, out_bytes, pitch, row_bytes);
   cudaStream_t st = ctx->stream;
   // pageable buffers go through the library's pinned staging (several copying threads)
@@ -3703,7 +3588,7 @@ extern "C" int rsb200_plan_run_gather(rsb200_plan* p, rsb200_comm* c, const void
   // the transfers start behind whatever the caller queued on `stream` so far
   CUDA_TRY(ctx, cudaEventRecord(c->done, st));
   CUDA_TRY(ctx, cudaStreamWaitEvent(c->stream, c->done, 0));
-  if (p->kind == 1 && !p->tile_groups.empty() && !p->host_tiles_only) {
+  if (p->kind == PlanKind::Ljpeg && !p->tile_groups.empty() && !p->host_tiles_only) {
     if (in_bytes < p->need_in)
       return set_err(ctx, RSB200_ERR_ARG, "plan_run_gather: input too small");
     while (c->events.size() < p->tile_groups.size()) {
@@ -3749,20 +3634,20 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
   rsb200_ctx* ctx = p->ctx;
   if (!p->ran)
     return set_err(ctx, RSB200_ERR_ARG, "plan_results: plan has not been run");
-  if (p->kind == 4 || p->kind == 6) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_arw2_bad, p->d_arw2_bad, sizeof(uint32_t) * (size_t)p->nunits,
+  if (p->kind == PlanKind::Arw2 || p->kind == PlanKind::PhaseOne) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_job_bad.get(), p->d_job_bad.get(), sizeof(uint32_t) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
     int first = RSB200_OK;
     for (int i = 0; i < p->nunits; ++i) {
-      const bool bad = p->h_arw2_bad[i] != 0;
+      const bool bad = p->h_job_bad[i] != 0;
       if (results && i < n) {
         results[i].status = bad ? RSB200_ERR_RDE : RSB200_OK;
         results[i].consumed = 0;
       }
       if (bad && first == RSB200_OK) {
         first = RSB200_ERR_RDE;
-        set_err(ctx, first, p->kind == 4
+        set_err(ctx, first, p->kind == PlanKind::Arw2
                                 ? "Too many errors encountered. Giving up. First Error:\n"
                                   "ARW2 invariant failed, same pixel is both min and max"
                                 : "Too many errors encountered. Giving up. First Error:\n"
@@ -3771,8 +3656,8 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
-  if (p->kind == 12) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_s0_res, p->d_s0_res, sizeof(uint2) * (size_t)p->nunits,
+  if (p->kind == PlanKind::SamsungV0) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_job_res.get(), p->d_job_res.get(), sizeof(uint2) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
     static const char* const msgs[7] = {"", "Bit length less than 0.", "Bit Length more than 16.",
@@ -3782,7 +3667,7 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
                                         "Bit stream size is smaller than MaxProcessBytes"};
     int first = RSB200_OK;
     for (int i = 0; i < p->nunits; ++i) {
-      const uint2 r = p->h_s0_res[i];
+      const uint2 r = p->h_job_res[i];
       if (results && i < n) {
         results[i].status = r.x;
         results[i].consumed = r.y;
@@ -3795,8 +3680,8 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
-  if (p->kind == 13) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_s0_res, p->d_s0_res, sizeof(uint2) * (size_t)p->nunits,
+  if (p->kind == PlanKind::SamsungV2) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_job_res.get(), p->d_job_res.get(), sizeof(uint2) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
     // SamsungV2Decompressor.cpp:180-247, 329-350; BitStreamer.h; ByteStream::check
@@ -3810,7 +3695,7 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
                                         "Out of bounds access in ByteStream"};
     int first = RSB200_OK;
     for (int i = 0; i < p->nunits; ++i) {
-      const uint2 r = p->h_s0_res[i];
+      const uint2 r = p->h_job_res[i];
       if (results && i < n) {
         results[i].status = r.x;
         results[i].consumed = r.y;
@@ -3824,8 +3709,8 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
-  if (p->kind == 11) {
-    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_hass_states, p->d_hass_states, sizeof(DevHassState) * (size_t)p->nunits,
+  if (p->kind == PlanKind::Hasselblad) {
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_hass_states.get(), p->d_hass_states.get(), sizeof(DevHassState) * (size_t)p->nunits,
                                   cudaMemcpyDeviceToHost, p->last_stream));
     CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
     int first = RSB200_OK;
@@ -3848,7 +3733,7 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return first;
   }
-  if (p->kind != 1) {
+  if (p->kind != PlanKind::Ljpeg) {
     CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
     for (int i = 0; results && i < n; ++i) {
       results[i].status = RSB200_OK;
@@ -3856,10 +3741,10 @@ extern "C" int rsb200_plan_results(rsb200_plan* p, rsb200_scan_result* results, 
     }
     return RSB200_OK;
   }
-  CUDA_TRY(ctx, cudaMemcpyAsync(p->h_results, p->d_results, sizeof(DevResult) * p->nscans,
+  CUDA_TRY(ctx, cudaMemcpyAsync(p->h_results.get(), p->d_results.get(), sizeof(DevResult) * p->nscans,
                                 cudaMemcpyDeviceToHost, p->last_stream));
   if (p->d_oob)
-    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_oob, p->d_oob, sizeof(uint32_t) * p->nscans,
+    CUDA_TRY(ctx, cudaMemcpyAsync(p->h_oob.get(), p->d_oob.get(), sizeof(uint32_t) * p->nscans,
                                   cudaMemcpyDeviceToHost, p->last_stream));
   CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
   int first = RSB200_OK;
@@ -3939,7 +3824,7 @@ extern "C" int rsb200_debug_range_redo(const rsb200_plan* p, uint32_t* flags, in
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
   std::vector<uint32_t> fb(p->h_big_ids.size());
-  CUDA_TRY(ctx, cudaMemcpy(fb.data(), p->d_fallback, sizeof(uint32_t) * fb.size(), cudaMemcpyDeviceToHost));
+  CUDA_TRY(ctx, cudaMemcpy(fb.data(), p->d_fallback.get(), sizeof(uint32_t) * fb.size(), cudaMemcpyDeviceToHost));
   for (size_t k = 0; k < fb.size(); ++k)
     if ((int)p->h_big_ids[k] < n)
       flags[p->h_big_ids[k]] = fb[k] ? 1u : 0u;
@@ -3952,22 +3837,22 @@ extern "C" int rsb200_plan_bad_pixels(rsb200_plan* p, int job, uint32_t* positio
     return RSB200_ERR_ARG;
   rsb200_ctx* ctx = p->ctx;
   *count = 0;
-  if ((p->kind != 5 && p->kind != 8) || job < 0 || job >= (int)p->pana_zero_slot.size())
+  if ((p->kind != PlanKind::Pana && p->kind != PlanKind::DngOp) || job < 0 || job >= (int)p->bad_slot.size())
     return set_err(ctx, RSB200_ERR_ARG,
                    "plan_bad_pixels: not a job of a Panasonic plan / an opcode of a DNG opcode plan");
   if (!p->ran)
     return set_err(ctx, RSB200_ERR_ARG, "plan_bad_pixels: plan has not been run");
-  const int slot = p->pana_zero_slot[job];
+  const int slot = p->bad_slot[job];
   if (slot < 0)
     return RSB200_OK; // zero_is_not_bad (or not V4): the reference collects nothing
   CUDA_TRY(ctx, cudaSetDevice(ctx->device));
   CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
   uint32_t n = 0;
-  CUDA_TRY(ctx, cudaMemcpy(&n, p->d_pana_zero_count + slot, sizeof n, cudaMemcpyDeviceToHost));
+  CUDA_TRY(ctx, cudaMemcpy(&n, p->d_bad_count.get() + slot, sizeof n, cudaMemcpyDeviceToHost));
   *count = n;
   const uint32_t take = std::min(std::min(n, cap), (uint32_t)PANA_ZERO_CAP);
   if (take && positions)
-    CUDA_TRY(ctx, cudaMemcpy(positions, p->d_pana_zero_list + (size_t)slot * PANA_ZERO_CAP,
+    CUDA_TRY(ctx, cudaMemcpy(positions, p->d_bad_list.get() + (size_t)slot * PANA_ZERO_CAP,
                              sizeof(uint32_t) * take, cudaMemcpyDeviceToHost));
   return RSB200_OK;
 }
@@ -3992,7 +3877,7 @@ extern "C" int rsb200_plan_launches(const rsb200_plan* p) {
 extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
   if (!p)
     return "";
-  if (p->kind == 0) {
+  if (p->kind == PlanKind::Unpack) {
     // jobs of bit depth 8/10/12/14/16 with 4-byte aligned input rows of >= 64 items (1024
     // samples) take the fast kernel, the others the generic one
     if (!p->fast_groups.empty() && !p->groups.empty())
@@ -4001,15 +3886,15 @@ extern "C" const char* rsb200_plan_kernels(const rsb200_plan* p) {
       return "unpack_fast_kernel";
     return p->groups.empty() ? "(empty unpack plan)" : "unpack_kernel";
   }
-  if (p->kind == 2)
+  if (p->kind == PlanKind::RawForm)
     return p->raw_groups.empty() ? "(empty raw-form plan)" : "rawform_kernel";
-  if (p->kind == 13)
+  if (p->kind == PlanKind::SamsungV2)
     return "s2_cand_kernel + s2_pair_kernel + s2_double_kernel + s2_coarse_kernel + s2_fine_kernel + s2_desc_kernel + "
            "s2_diff_kernel + s2_recon_kernel";
-  if (p->kind == 12)
+  if (p->kind == PlanKind::SamsungV0)
     return "s0_walk_kernel + s0_diff_kernel + s0_node_kernel + s0_jump_kernel + s0_scan_kernel + s0_carry_kernel + "
            "s0_store_kernel";
-  if (p->kind != 1)
+  if (p->kind != PlanKind::Ljpeg)
     return "(not an LJPEG plan)";
   const bool only_thread = p->nthread && !p->ntile && !p->nsmall && !p->nbig;
   const bool only_tile = p->ntile && !p->nthread && !p->nsmall && !p->nbig;
@@ -4041,107 +3926,6 @@ extern "C" void rsb200_plan_destroy(rsb200_plan* p) {
   if (p->ctx)
     cudaSetDevice(p->ctx->device);
   if (p->ran && p->last_stream)
-    cudaStreamSynchronize(p->last_stream); // (the frees below are stream ordered, not device-wide syncs)
-  for (UnpackGroup& g : p->groups)
-    rsb_dev_free(g.d_jobs);
-  for (UnpackFastGroup& g : p->fast_groups)
-    rsb_dev_free(g.d_jobs);
-  for (RawGroup& g : p->raw_groups)
-    rsb_dev_free(g.d_jobs);
-  for (PanaGroup& g : p->pana_groups)
-    rsb_dev_free(g.d_jobs);
-  for (ScaleGroup& g : p->scale_groups)
-    rsb_dev_free(g.d_jobs);
-  rsb_dev_free(p->d_pana_zero_count);
-  rsb_dev_free(p->d_pana_zero_list);
-  rsb_dev_free(p->d_lookup_jobs);
-  rsb_dev_free(p->d_lookup_tables);
-  rsb_dev_free(p->d_badpix_jobs);
-  rsb_dev_free(p->d_badpix_list);
-  rsb_dev_free(p->d_badpix_maps);
-  rsb_dev_free(p->d_dngop_jobs);
-  rsb_dev_free(p->d_dngop_ops);
-  rsb_dev_free(p->d_dngop_tables);
-  rsb_dev_free(p->d_dngop_deltas);
-  rsb_dev_free(p->d_hass_jobs);
-  rsb_dev_free(p->d_hass_ctas);
-  rsb_dev_free(p->d_hass_states);
-  rsb_host_free(p->h_hass_states);
-  rsb_dev_free(p->d_hass_seg_job);
-  rsb_dev_free(p->d_hass_u32);
-  rsb_dev_free(p->d_hass_row_begin);
-  rsb_dev_free(p->d_s0_rows);
-  rsb_dev_free(p->d_s0_jobs);
-  rsb_dev_free(p->d_s0_desc);
-  rsb_dev_free(p->d_s0_adj);
-  rsb_dev_free(p->d_s0_nodes);
-  rsb_dev_free(p->d_s0_carry);
-  rsb_dev_free(p->d_s0_rowfail);
-  rsb_dev_free(p->d_s0_jobfail);
-  rsb_dev_free(p->d_s0_res);
-  rsb_dev_free(p->d_s2_frames);
-  rsb_dev_free(p->d_s2_starts);
-  rsb_dev_free(p->d_s2_tab);
-  rsb_dev_free(p->d_s2_jump);
-  rsb_dev_free(p->d_s2_rowstart);
-  rsb_dev_free(p->d_s2_cp);
-  rsb_dev_free(p->d_s2_ncp);
-  rsb_dev_free(p->d_s2_fail);
-  rsb_dev_free(p->d_s2_desc);
-  rsb_dev_free(p->d_s2_px);
-  if (p->h_s0_res)
-    rsb_host_free(p->h_s0_res);
-  rsb_dev_free(p->d_p1_strips);
-  rsb_dev_free(p->d_p1_jobs);
-  rsb_dev_free(p->d_p1_gdesc);
-  rsb_dev_free(p->d_p1_rowflag);
-  rsb_dev_free(p->d_nikon_luts);
-  rsb_dev_free(p->d_arw2_jobs);
-  rsb_dev_free(p->d_arw2_tables);
-  rsb_dev_free(p->d_arw2_bad);
-  if (p->h_arw2_bad)
-    rsb_host_free(p->h_arw2_bad);
-  for (SrawGroup& g : p->sraw_groups)
-    rsb_dev_free(g.d_jobs);
-  rsb_dev_free(p->d_raw_tables);
-  rsb_dev_free(p->d_tables);
-  rsb_dev_free(p->d_scans);
-  rsb_dev_free(p->d_strips);
-  rsb_dev_free(p->d_rows);
-  rsb_dev_free(p->d_diffs);
-  rsb_dev_free(p->d_colvals);
-  rsb_dev_free(p->d_results);
-  rsb_dev_free(p->d_small_ids);
-  rsb_dev_free(p->d_tile_ids);
-  rsb_dev_free(p->d_tile_params);
-  rsb_dev_free(p->d_thread_tile_params);
-  rsb_dev_free(p->d_redo);
-  rsb_dev_free(p->d_thread_ids);
-  rsb_dev_free(p->d_tscans);
-  rsb_dev_free(p->d_tinfos);
-  rsb_dev_free(p->d_clean);
-  rsb_dev_free(p->d_anchors);
-  rsb_dev_free(p->d_big_ids);
-  rsb_dev_free(p->d_big);
-  rsb_dev_free(p->d_ranges);
-  rsb_dev_free(p->d_states);
-  rsb_dev_free(p->d_finals);
-  rsb_dev_free(p->d_fallback);
-  rsb_dev_free(p->d_oob);
-  rsb_dev_free(p->d_arw1);
-  rsb_dev_free(p->d_arw1_in);
-  rsb_dev_free(p->d_arw1_runs);
-  rsb_dev_free(p->d_arw1_lastoff);
-  rsb_dev_free(p->d_arw1_runpre);
-  rsb_dev_free(p->d_arw1_info);
-  rsb_dev_free(p->d_s1);
-  rsb_dev_free(p->d_s1_colvals);
-  rsb_dev_free(p->d_s1_rowbits);
-  rsb_dev_free(p->d_s1_oob);
-  rsb_dev_free(p->d_s1_lim);
-  if (p->h_oob)
-    rsb_host_free(p->h_oob);
-  if (p->h_results)
-    rsb_host_free(p->h_results);
+    cudaStreamSynchronize(p->last_stream); // (the owners free stream ordered, not with device-wide syncs)
   delete p;
 }
