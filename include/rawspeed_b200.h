@@ -651,6 +651,47 @@ int rsb200_samsung2_plan_create(rsb200_ctx* ctx, const rsb200_samsung2_job* jobs
                                 rsb200_plan** plan);
 
 /* ------------------------------------------------------------------ */
+/* Kodak DCR, compression 65000 (DESIGN 8(f)4).                          */
+/*   KodakDecompressor::KodakDecompressor / decompress                   */
+/*   decompressors/KodakDecompressor.cpp:46-150                          */
+/*   (rows cut into segments of up to 256 pixels; a segment is a header  */
+/*   of 4-bit lengths, then the differences as a bit string, predicted   */
+/*   per parity from 0 at every segment).                                */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint64_t in_offset;  /* first byte of the stream                                 */
+  uint32_t in_size;    /* bytes of the stream; <= 2^28                             */
+  int32_t width;       /* the RawImage's dimensions                                */
+  int32_t height;
+  int32_t bps;         /* bits per sample (10 or 12)                               */
+  int32_t table;       /* index into the plan's tables, -1 = none (uncorrectedRawValues,
+                          or an image without a table)                             */
+  uint64_t out_offset; /* byte offset of image row 0; multiple of 4                */
+  uint32_t out_pitch;  /* bytes; multiple of 4, >= 2 * width                       */
+  uint32_t reserved;   /* 0                                                        */
+} rsb200_kodak_job;
+
+/* `tables`: ntables x 65536 uint16 entries, as for rsb200_raw_plan_create (for a dithered table pass
+ * entries 2*v: the dither counter of decompress starts at 0 and stays there, RawImage.h:335-353).
+ * Plan creation runs the constructor's checks in its order (KodakDecompressor.cpp:50-64): dimensions
+ * (RSB200_ERR_RDE "Unexpected image dimensions found: (%d; %d)"), bps ("Unexpected bits per sample: %i"),
+ * then in_size < width * height / 2 (RSB200_ERR_IOE "Out of bounds access in ByteStream").  An
+ * out_offset or out_pitch that is not a multiple of 4, a pitch below 2 * width, in_size > 2^28, a table
+ * outside 0..ntables - 1 (other than -1) or a non-zero reserved field are refused with RSB200_ERR_ARG.
+ * rsb200_plan_results() per job: RSB200_ERR_RDE or RSB200_ERR_IOE with consumed ==
+ * code << 28 | row << 13 | column, code one of RSB200_KODAK_*, column the failing pixel's (RDE) or the
+ * first of the segment that reads past the end (IOE).  The image then holds every pixel in front of
+ * that one in raster order and nothing else.  The value the RDE message prints comes from
+ * rsb200_kodak_plan_values. */
+#define RSB200_KODAK_VALUE 1u    /* RDE "Value out of bounds %d (bps = %i)"          */
+#define RSB200_KODAK_OVERFLOW 2u /* IOE "Buffer overflow: image file may be truncated" */
+int rsb200_kodak_plan_create(rsb200_ctx* ctx, const rsb200_kodak_job* jobs, int njobs, const uint16_t* tables,
+                             int ntables, rsb200_plan** plan);
+/* After a run of a Kodak plan: values[i] (i < n) = the value job i's RSB200_KODAK_VALUE failure prints,
+ * 0 for a job without one.  RSB200_ERR_ARG for another kind of plan or one that has not run. */
+int rsb200_kodak_plan_values(rsb200_plan* plan, int32_t* values, int n);
+
+/* ------------------------------------------------------------------ */
 /* Nikon NEF Huffman codec without split (SURVEY 8(f)2).                 */
 /*   NikonDecompressor::decompress  decompressors/NikonDecompressor.cpp:513-560 */
 /*   (plain MSB bit stream, nikon_tree table, per-parity left predictor, */

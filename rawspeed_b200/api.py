@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, SamsungV2Job, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, SamsungV2Job, KodakJob, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -162,6 +162,13 @@ class Plan:
         n = C.c_uint32(0)
         self.ctx.check(self.ctx._lib.rsb200_plan_bad_pixels(self.h, job, buf, cap, C.byref(n)))
         return n.value, list(buf[:min(n.value, cap)])
+
+    def kodak_values(self):
+        """Kodak plan after a run: per job, the value its "Value out of bounds" failure prints (0 for
+        a job without one)."""
+        buf = (C.c_int32 * self.nunits)()
+        self.ctx.check(self.ctx._lib.rsb200_kodak_plan_values(self.h, buf, self.nunits))
+        return list(buf)
 
     @property
     def launches(self):
@@ -384,6 +391,22 @@ def samsung2_plan(ctx, jobs):
     ja = (SamsungV2Job * len(jobs))(*jobs)
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_samsung2_plan_create(ctx.h, ja, len(jobs), C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def kodak_plan(ctx, jobs, tables=None):
+    """Kodak DCR streams (KodakDecompressor::decompress), one job per frame.  tables: None or a
+    (n, 65536) uint16 array (for a dithered RawImage table, its entries 2*v); job.table indexes it
+    (-1 = none).  After a run, plan.kodak_values() gives the value each job's "Value out of bounds"
+    prints."""
+    ja = (KodakJob * len(jobs))(*jobs)
+    if tables is None:
+        tp, nt = None, 0
+    else:
+        t = np.ascontiguousarray(tables, dtype=np.uint16).reshape(-1, 65536)
+        tp, nt = t.ctypes.data, t.shape[0]
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_kodak_plan_create(ctx.h, ja, len(jobs), tp, nt, C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

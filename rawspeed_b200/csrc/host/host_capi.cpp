@@ -384,6 +384,25 @@ int rsb200h_samsung_v2(uint16_t* img_data, int w, int h, int cpp, int pitch, con
   });
 }
 
+// cpp: components per pixel of the image (the constructor refuses anything but 1); curve != NULL ->
+// mRaw->setTable(curve, dither) first
+int rsb200h_kodak(uint16_t* img_data, int w, int h, int cpp, int pitch, const uint8_t* data, uint32_t size, int bps,
+                  int uncorrected, const uint16_t* curve, int ncurve, int dither, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, cpp, pitch, true, 1, 1);
+    if (curve)
+      img->setTable(std::vector<uint16_t>(curve, curve + ncurve), dither != 0);
+    KodakDecompressor d(img, ByteStream(data, size), bps, uncorrected != 0);
+    try {
+      d.decompress();
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
                                  uint32_t size, rsb200h_err* e) {
   return guarded(e, [&] {

@@ -935,6 +935,68 @@ void SamsungV2Decompressor::decompress() const {
   }
 }
 
+// ------------------------------------------------------------------ Kodak DCR
+KodakDecompressor::KodakDecompressor(RawImage img, ByteStream bs, int bps_, bool uncorrectedRawValues_)
+    : mRaw(std::move(img)), input(bs), bps(bps_), uncorrectedRawValues(uncorrectedRawValues_) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||
+      mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  if (!mRaw->dim.hasPositiveArea() || mRaw->dim.x % 4 != 0 || mRaw->dim.x > 4516 || mRaw->dim.y > 3012)
+    ThrowRDE("Unexpected image dimensions found: (%d; %d)", mRaw->dim.x, mRaw->dim.y);
+  if (bps != 10 && bps != 12)
+    ThrowRDE("Unexpected bits per sample: %i", bps);
+  // Lower estimate: this decompressor requires *at least* half a byte per output pixel
+  (void)input.check((uint32_t)((uint64_t)mRaw->dim.area() / 2ULL));
+}
+
+void KodakDecompressor::decompress() const {
+  rsb200_kodak_job job;
+  std::memset(&job, 0, sizeof job);
+  job.in_offset = 0;
+  // A row reads at most 608 bytes per full segment (128 of lengths, 4 * ceil(15 * 256 / 32) of
+  // differences) and the tail's maximum; more data behind that changes no outcome.
+  const uint32_t w = (uint32_t)mRaw->dim.x, t = w % 256u, e = (t & 7u) == 4u ? 2u : 0u;
+  const uint64_t tailMax = t ? t / 2u + e + 4u * ((15u * t > 8u * e ? 15u * t - 8u * e + 31u : 0u) / 32u) : 0u;
+  const uint64_t most = (uint64_t)mRaw->dim.y * (608ull * (w / 256u) + tailMax);
+  job.in_size = (uint32_t)std::min<uint64_t>(input.getRemainSize(), most);
+  job.width = mRaw->dim.x;
+  job.height = mRaw->dim.y;
+  job.bps = bps;
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  // setWithLookUp (RawImage.h:335-353): the dither counter starts at 0 and stays there, so a dithered
+  // table reads entry 2 * v exactly; the device gets one 65536-entry table either way
+  const bool lut = !uncorrectedRawValues && mRaw->hasTable();
+  std::vector<uint16_t> dev;
+  if (lut) {
+    const std::vector<uint16_t>& tab = mRaw->tableData();
+    dev.resize(65536);
+    for (int i = 0; i < 65536; ++i)
+      dev[i] = mRaw->tableDither() ? tab[(size_t)2 * i] : tab[i];
+  }
+  job.table = lut ? 0 : -1;
+  PlanGuard pg;
+  engineCheck(rsb200_kodak_plan_create(engine(), &job, 1, lut ? dev.data() : nullptr, lut ? 1 : 0, &pg.p),
+              "rsb200_kodak_plan_create");
+  RawImage img = mRaw;
+  runOnImage(pg.p, input.begin() + input.getPosition(), job.in_size, img, /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  switch (res.consumed >> 28) { // KodakDecompressor.cpp:137-138; Buffer.h:78-83
+  case RSB200_KODAK_VALUE: {
+    int32_t value = 0;
+    engineCheck(rsb200_kodak_plan_values(pg.p, &value, 1), "rsb200_kodak_plan_values");
+    ThrowRDE("Value out of bounds %d (bps = %i)", (int)value, bps);
+  }
+  case RSB200_KODAK_OVERFLOW:
+    ThrowIOE("Buffer overflow: image file may be truncated");
+  default:
+    engineCheck(rc, "rsb200_plan_results");
+  }
+}
+
 // ------------------------------------------------------------------ Sony ARW1
 SonyArw1Decompressor::SonyArw1Decompressor(RawImage img) : mRaw(std::move(img)) {
   if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 ||

@@ -627,6 +627,23 @@ private:
   unsigned bits;
 };
 
+// ---------------------------------------------------------------- Kodak DCR
+// decompressors/KodakDecompressor.h: same constructor (image, stream, bits per sample,
+// uncorrectedRawValues; its checks, KodakDecompressor.cpp:46-65, in its order) and decompress().  The
+// segments are decoded on the device (kodak.cuh) through the image's table (none, plain or dithered);
+// errors are thrown with the reference's classes and messages, printed values included.
+class KodakDecompressor final {
+public:
+  KodakDecompressor(RawImage img, ByteStream bs, int bps, bool uncorrectedRawValues);
+  void decompress() const;
+
+private:
+  RawImage mRaw;
+  ByteStream input;
+  int bps;
+  bool uncorrectedRawValues;
+};
+
 // ---------------------------------------------------------------- Sony ARW1
 // decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
 // SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs

@@ -32,6 +32,7 @@
 #include "samsung0.cuh"
 #include "samsung1.cuh"
 #include "samsung2.cuh"
+#include "kodak.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -383,6 +384,27 @@ struct SamsungV2Plan {
   PinnedPtr<uint2> h_job_res;
 };
 
+// Kodak DCR (kodak.cuh)
+struct KodakPlan {
+  DevPtr<KdFrameDev> d_kd_frames;
+  DevPtr<uint32_t> d_kd_starts; // per frame, four searches: tiles, candidates, checkpoints, segments
+  DevPtr<uint16_t> d_kd_tables;
+  DevPtr<uint32_t> d_kd_tsum;   // per prefix tile
+  DevPtr<uint32_t> d_kd_q;      // nibble-sum prefix
+  DevPtr<uint32_t> d_kd_tab;    // candidate entries
+  DevPtr<uint32_t> d_kd_jump;   // two ping-pong buffers of kd_ncand
+  DevPtr<uint32_t> d_kd_rowstart;
+  DevPtr<uint32_t> d_kd_cp;
+  DevPtr<uint32_t> d_kd_ncp;
+  DevPtr<uint2> d_kd_fail;
+  DevPtr<uint32_t> d_kd_key;
+  uint32_t kd_ntiles = 0, kd_ncand = 0, kd_ncp = 0, kd_nsegs = 0;
+  // per-job results and printed values
+  DevPtr<uint2> d_job_res;
+  PinnedPtr<uint2> h_job_res;
+  DevPtr<int32_t> d_kd_values;
+};
+
 // Sony ARW2
 struct Arw2Plan {
   DevPtr<Arw2JobDev> d_arw2_jobs;
@@ -489,7 +511,7 @@ struct rsb200_plan {
   cudaStream_t last_stream = nullptr;
   bool ran = false;
   std::variant<UnpackPlan, LjpegPlan, RawFormPlan, SrawPlan, Arw2Plan, PanaPlan, PhaseOnePlan, ScalePlan, DngOpPlan,
-               BadPixPlan, LookupPlan, HasselbladPlan, SamsungV0Plan, SamsungV2Plan>
+               BadPixPlan, LookupPlan, HasselbladPlan, SamsungV0Plan, SamsungV2Plan, KodakPlan>
       state;
 };
 
@@ -1935,6 +1957,143 @@ static int results(const rsb200_plan* p, SamsungV2Plan& s, rsb200_scan_result* o
 static const char* kernels(const rsb200_plan*, const SamsungV2Plan&) {
   return "s2_cand_kernel + s2_pair_kernel + s2_double_kernel + s2_coarse_kernel + s2_fine_kernel + s2_desc_kernel + "
          "s2_diff_kernel + s2_recon_kernel";
+}
+
+// ------------------------------------------------------------------
+// Kodak DCR: segments of up to 256 pixels, row starts resolved from every candidate (kodak.cuh)
+// ------------------------------------------------------------------
+extern "C" int rsb200_kodak_plan_create(rsb200_ctx* ctx, const rsb200_kodak_job* jobs, int njobs,
+                                        const uint16_t* tables, int ntables, rsb200_plan** out) {
+  if (!ctx || !jobs || njobs <= 0 || ntables < 0 || (ntables > 0 && !tables) || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "kodak_plan_create: bad arguments");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_kodak_job& j = jobs[i];
+    // KodakDecompressor ctor (KodakDecompressor.cpp:50-64), in its order
+    if (j.width <= 0 || j.height <= 0 || j.width % 4 != 0 || j.width > (int32_t)KD_MAXW || j.height > (int32_t)KD_MAXH)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected image dimensions found: (%d; %d)", i, j.width, j.height);
+    if (j.bps != 10 && j.bps != 12)
+      return set_err(ctx, RSB200_ERR_RDE, "job %d: Unexpected bits per sample: %i", i, j.bps);
+    if ((uint64_t)j.in_size < (uint64_t)j.width * (uint64_t)j.height / 2u)
+      return set_err(ctx, RSB200_ERR_IOE, "job %d: Out of bounds access in ByteStream", i);
+    // the stores write two pixels as one 32-bit word
+    if (j.in_size > KD_MAX_IN || (uint64_t)j.width * 2 > j.out_pitch || (j.out_offset % 4) || (j.out_pitch % 4) ||
+        j.table < -1 || j.table >= ntables || j.reserved)
+      return set_err(ctx, RSB200_ERR_ARG, "kodak job %d: malformed descriptor", i);
+  }
+  PlanHolder holder = new_plan(ctx);
+  if (!holder)
+    return RSB200_ERR_CUDA;
+  rsb200_plan* p = holder.get();
+  KodakPlan& s = p->state.emplace<KodakPlan>();
+  p->nunits = njobs;
+  std::vector<KdFrameDev> fr((size_t)njobs);
+  std::vector<uint32_t> starts((size_t)njobs * 4);
+  KdTotals t;
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_kodak_job& j = jobs[i];
+    kd_place_frame(fr[(size_t)i], t, starts.data(), (uint32_t)njobs, (uint32_t)i, j.in_offset, j.in_size,
+                   (uint32_t)j.width, (uint32_t)j.height, (uint32_t)j.bps,
+                   j.table < 0 ? ~0u : (uint32_t)j.table * 65536u, j.out_offset, j.out_pitch);
+    if (t.q >= (1ull << 31) || t.cand >= (1ull << 31) || t.segs >= (1ull << 31))
+      return set_err(ctx, RSB200_ERR_ARG, "kodak plan: too many frames for one plan");
+    p->in_bytes += j.in_size;
+    p->out_bytes += (uint64_t)j.width * j.height * 2;
+    p->pixels += (uint64_t)j.width * j.height;
+    p->need_in = std::max<uint64_t>(p->need_in, sat_add(j.in_offset, j.in_size));
+    p->need_out = std::max<uint64_t>(p->need_out,
+                                     sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch + 2ull * j.width));
+  }
+  s.kd_ntiles = (uint32_t)t.tiles;
+  s.kd_ncand = (uint32_t)t.cand;
+  s.kd_ncp = (uint32_t)t.cps;
+  s.kd_nsegs = (uint32_t)t.segs;
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, s.d_kd_frames, fr.data(), sizeof(KdFrameDev) * fr.size());
+  dev_upload(e, s.d_kd_starts, starts.data(), sizeof(uint32_t) * starts.size());
+  dev_upload(e, s.d_kd_tables, tables, sizeof(uint16_t) * 65536 * (size_t)ntables);
+  dev_alloc(e, s.d_kd_tsum, sizeof(uint32_t) * t.tiles);
+  dev_alloc(e, s.d_kd_q, sizeof(uint32_t) * t.q);
+  dev_alloc(e, s.d_kd_tab, sizeof(uint32_t) * t.cand);
+  dev_alloc(e, s.d_kd_jump, sizeof(uint32_t) * 2 * t.cand);
+  dev_alloc(e, s.d_kd_rowstart, sizeof(uint32_t) * t.rows);
+  dev_alloc(e, s.d_kd_cp, sizeof(uint32_t) * t.cps);
+  dev_alloc(e, s.d_kd_ncp, sizeof(uint32_t) * (size_t)njobs);
+  dev_alloc(e, s.d_kd_fail, sizeof(uint2) * (size_t)njobs);
+  dev_alloc(e, s.d_kd_key, sizeof(uint32_t) * (size_t)njobs);
+  dev_alloc(e, s.d_job_res, sizeof(uint2) * (size_t)njobs);
+  host_alloc(e, s.h_job_res, sizeof(uint2) * (size_t)njobs);
+  dev_alloc(e, s.d_kd_values, sizeof(int32_t) * (size_t)njobs);
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "kodak plan allocation failed: %s", cudaGetErrorString(e));
+  p->launches_per_run = 8 + KD_JUMP;
+  *out = holder.release();
+  return RSB200_OK;
+}
+
+static int run(const rsb200_plan* p, const KodakPlan& s, const uint8_t* in, uint64_t, uint8_t* outp, cudaStream_t st) {
+  const uint32_t nf = (uint32_t)p->nunits;
+  const uint32_t* starts = s.d_kd_starts.get();
+  const KdFrameDev* fr = s.d_kd_frames.get();
+  kd_tsum_kernel<<<s.kd_ntiles, KD_NT, 0, st>>>(in, fr, starts, nf, s.d_kd_tsum.get());
+  kd_tscan_kernel<<<nf, KD_NT, 0, st>>>(fr, s.d_kd_tsum.get());
+  kd_prefix_kernel<<<s.kd_ntiles, KD_NT, 0, st>>>(in, fr, starts, nf, s.d_kd_tsum.get(), s.d_kd_q.get());
+  const uint32_t gc = (s.kd_ncand + KD_NT - 1) / KD_NT;
+  kd_cand_kernel<<<gc, KD_NT, 0, st>>>(fr, starts + nf, nf, s.kd_ncand, s.d_kd_q.get(), s.d_kd_tab.get());
+  const uint32_t* src = s.d_kd_tab.get();
+  uint32_t* dst = s.d_kd_jump.get();
+  for (int r = 0; r < KD_JUMP; ++r) {
+    kd_double_kernel<<<gc, KD_NT, 0, st>>>(fr, starts + nf, nf, s.kd_ncand, src, dst);
+    src = dst;
+    dst = dst == s.d_kd_jump.get() ? s.d_kd_jump.get() + s.kd_ncand : s.d_kd_jump.get();
+  }
+  kd_coarse_kernel<<<(nf + KD_NT - 1) / KD_NT, KD_NT, 0, st>>>(fr, nf, src, s.d_kd_cp.get(), s.d_kd_ncp.get(),
+                                                               s.d_kd_fail.get(), s.d_kd_key.get());
+  kd_fine_kernel<<<(s.kd_ncp + KD_NT - 1) / KD_NT, KD_NT, 0, st>>>(fr, starts + 2 * nf, nf, s.kd_ncp, s.d_kd_tab.get(),
+                                                                   s.d_kd_cp.get(), s.d_kd_ncp.get(),
+                                                                   s.d_kd_rowstart.get(), s.d_kd_fail.get());
+  const uint32_t gs = (s.kd_nsegs + KD_NT / 32 - 1) / (KD_NT / 32);
+  kd_check_kernel<<<gs, KD_NT, 0, st>>>(in, fr, starts + 3 * nf, nf, s.kd_nsegs, s.d_kd_q.get(), s.d_kd_rowstart.get(),
+                                        s.d_kd_fail.get(), s.d_kd_key.get());
+  kd_store_kernel<<<gs, KD_NT, 0, st>>>(in, fr, starts + 3 * nf, nf, s.kd_nsegs, s.d_kd_q.get(), s.d_kd_rowstart.get(),
+                                        s.d_kd_fail.get(), s.d_kd_key.get(), s.d_kd_tables.get(), outp,
+                                        s.d_job_res.get(), s.d_kd_values.get());
+  CUDA_TRY(p->ctx, cudaGetLastError());
+  p->ctx->launches += (uint64_t)p->launches_per_run;
+  return RSB200_OK;
+}
+
+static int results(const rsb200_plan* p, KodakPlan& s, rsb200_scan_result* out, int n) {
+  // KodakDecompressor.cpp:137-138; Buffer.h:78-83
+  return report_jobs(
+      p, s.d_job_res, s.h_job_res, out, n, [&](int i) { return rsb200_scan_result{s.h_job_res[i].x, s.h_job_res[i].y}; },
+      [&](int i, const rsb200_scan_result& r) {
+        set_err(p->ctx, (int)r.status, "job %d: %s (row %u, column %u)", i,
+                r.status == RSB200_ERR_RDE ? "Value out of bounds" : "Buffer overflow: image file may be truncated",
+                (r.consumed >> 13) & 0x7FFFu, r.consumed & 0x1FFFu);
+      });
+}
+
+static const char* kernels(const rsb200_plan*, const KodakPlan&) {
+  return "kd_tsum_kernel + kd_tscan_kernel + kd_prefix_kernel + kd_cand_kernel + kd_double_kernel + kd_coarse_kernel + "
+         "kd_fine_kernel + kd_check_kernel + kd_store_kernel";
+}
+
+extern "C" int rsb200_kodak_plan_values(rsb200_plan* p, int32_t* values, int n) {
+  if (!p || (n > 0 && !values))
+    return RSB200_ERR_ARG;
+  rsb200_ctx* ctx = p->ctx;
+  const KodakPlan* s = std::get_if<KodakPlan>(&p->state);
+  if (!s)
+    return set_err(ctx, RSB200_ERR_ARG, "kodak_plan_values: not a Kodak plan");
+  if (!p->ran)
+    return set_err(ctx, RSB200_ERR_ARG, "kodak_plan_values: plan has not been run");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  CUDA_TRY(ctx, cudaStreamSynchronize(p->last_stream));
+  const int take = std::min(n, p->nunits);
+  if (take > 0)
+    CUDA_TRY(ctx, cudaMemcpy(values, s->d_kd_values.get(), sizeof(int32_t) * (size_t)take, cudaMemcpyDeviceToHost));
+  return RSB200_OK;
 }
 
 // ------------------------------------------------------------------
