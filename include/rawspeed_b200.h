@@ -692,6 +692,63 @@ int rsb200_kodak_plan_create(rsb200_ctx* ctx, const rsb200_kodak_job* jobs, int 
 int rsb200_kodak_plan_values(rsb200_plan* plan, int32_t* values, int n);
 
 /* ------------------------------------------------------------------ */
+/* GoPro VC-5, DNG compression 9 (DESIGN 4 VC5).                         */
+/*   VC5Decompressor::decode  decompressors/VC5Decompressor.cpp:137-960  */
+/*   (4 channels x 10 subbands: a low-pass band of fixed-width values    */
+/*   and nine run-length / prefix-code bands per channel, three inverse  */
+/*   wavelet levels, a Bayer combine through a log table).  The tag walk */
+/*   (parseVC5) runs on the host: a plan sees band payloads only.        */
+/* ------------------------------------------------------------------ */
+typedef struct {
+  uint32_t size;  /* code length in bits, 1..26                         */
+  uint32_t bits;  /* code word, right-justified                         */
+  uint32_t count; /* run length, 0..511 (0: a marker)                   */
+  uint32_t value; /* run value magnitude, 0..255 (decompanded by the plan) */
+} rsb200_vc5_code;
+
+typedef struct {
+  uint64_t in_offset; /* first byte of the band's payload                            */
+  uint32_t in_size;   /* bytes; high pass: a multiple of 4, <= 2^28; low pass: at least
+                         8 * ceil(w * h * precision / 64)                            */
+  int32_t param;      /* high pass: quantization (-32768..32767); low pass: precision 8..16 */
+} rsb200_vc5_band;
+
+typedef struct {
+  int32_t width;         /* the image: even, 34..65534 (a level-3 band of 3 or more)  */
+  int32_t height;
+  int32_t output_bits;   /* bit length of the white level, 1..16                      */
+  int32_t phase;         /* RSB200_VC5_RGGB or RSB200_VC5_GBRG                        */
+  uint8_t prescale[4][3]; /* [channel][wavelet 1..3]: PrescaleShift, 0..3 (2: descale) */
+  uint32_t first_band;   /* its 40 bands are bands[first_band + channel * 10 + subband] */
+  uint64_t out_offset;   /* byte offset of image row 0; multiple of 4                 */
+  uint32_t out_pitch;    /* bytes; multiple of 4, >= 2 * width                        */
+  uint32_t reserved;     /* 0                                                         */
+} rsb200_vc5_job;
+
+/* `codes`: ncodes entries, a complete prefix code (the Kraft sum is exactly 1, no code is a prefix of
+ * another), each size 1..26, count <= 511, value <= 255; else RSB200_ERR_ARG.  The plan builds its
+ * decode tables and decompanded values from it.  Refused with RSB200_ERR_ARG: a job whose width or
+ * height is odd, <= 32 (the reference reads outside its bands there) or > 65534, output_bits outside
+ * 1..16, a phase other than the two, a prescale > 3, bands outside 0..nbands - 1, an out_offset or
+ * out_pitch that is not a multiple of 4, a pitch below 2 * width, a non-zero reserved field, or a band
+ * that breaks the in_size / param rules above.
+ * rsb200_plan_results() per job: RSB200_ERR_RDE or RSB200_ERR_IOE (the two RSB200_VC5_* marked IOE)
+ * with consumed == code << 28 | channel << 4 | subband of the band the reference's decode (one worker)
+ * meets first among the failing ones: subbands 3, 2, 1, 6, 5, 4, 9, 8, 7, each for channels 0..3.
+ * Within a band, the failure is that of the first failing symbol in stream order.  A failed job's
+ * image is left untouched. */
+#define RSB200_VC5_RGGB 0
+#define RSB200_VC5_GBRG 2
+#define RSB200_VC5_QUANT 1u     /* RDE "Impossible RLV value given current quantum"          */
+#define RSB200_VC5_EARLY_END 2u /* RDE "Got EndOfBand marker while looking for next pixel"   */
+#define RSB200_VC5_OVERRUN 3u   /* RDE "Not all pixels consumed?"                            */
+#define RSB200_VC5_NO_END 4u    /* RDE "EndOfBand marker not found"                          */
+#define RSB200_VC5_SHORT 5u     /* IOE "Bit stream size is smaller than MaxProcessBytes"     */
+#define RSB200_VC5_OVERREAD 6u  /* IOE "Buffer overflow read in BitStreamer"                 */
+int rsb200_vc5_plan_create(rsb200_ctx* ctx, const rsb200_vc5_code* codes, int ncodes, const rsb200_vc5_job* jobs,
+                           int njobs, const rsb200_vc5_band* bands, int nbands, rsb200_plan** plan);
+
+/* ------------------------------------------------------------------ */
 /* Nikon NEF Huffman codec without split (SURVEY 8(f)2).                 */
 /*   NikonDecompressor::decompress  decompressors/NikonDecompressor.cpp:513-560 */
 /*   (plain MSB bit stream, nikon_tree table, per-parity left predictor, */

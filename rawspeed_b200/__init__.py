@@ -10,13 +10,13 @@ per-pixel decode hot path of darktable-org/rawspeed.
 Nothing in this package imports oracle/ (the CPU checker).  There is no CPU
 fallback: without the CUDA library and a GPU the API raises."""
 from .api import (Context, Plan, Rsb200Error, RawDecoderException, IOException,  # noqa: F401
-                  huff_table, unpack_plan, raw_plan, sraw_plan, SrawJob, arw2_plan, Arw2Job, nikon_plan, NikonJob, pana_plan, PanaJob, scale_plan, ScaleJob, dngop_plan, DngOp, DngOpJob, badpix_plan, BadPixJob, lookup_plan, LookupJob, phaseone_plan, PhaseOneJob, PhaseOneStrip, samsung0_plan, SamsungV0Job, SamsungV0Strip, samsung1_plan, SamsungV1Job, samsung2_plan, SamsungV2Job, kodak_plan, KodakJob, hasselblad_plan, HasselbladJob, pentax_plan, PentaxJob, arw1_plan, Arw1Job, ljpeg_plan, cr2_plan, image_pitch,
+                  huff_table, unpack_plan, raw_plan, sraw_plan, SrawJob, arw2_plan, Arw2Job, nikon_plan, NikonJob, pana_plan, PanaJob, scale_plan, ScaleJob, dngop_plan, DngOp, DngOpJob, badpix_plan, BadPixJob, lookup_plan, LookupJob, phaseone_plan, PhaseOneJob, PhaseOneStrip, samsung0_plan, SamsungV0Job, SamsungV0Strip, samsung1_plan, SamsungV1Job, samsung2_plan, SamsungV2Job, kodak_plan, KodakJob, vc5_plan, Vc5Job, Vc5Band, Vc5Code, hasselblad_plan, HasselbladJob, pentax_plan, PentaxJob, arw1_plan, Arw1Job, ljpeg_plan, cr2_plan, image_pitch,
                   new_image, RawJob, UnpackJob, LJpegScan, Cr2Job, HuffTable, LSB, MSB, MSB16, MSB32,
                   Comm, comm_unique_id, GATHER_NONE, GATHER_ALL, GATHER_ROOT)
 from . import _abi as formats  # noqa: F401  (formats.RAW_* constants)
 from . import build as _build  # noqa: F401
 
 __all__ = ["Context", "Plan", "Rsb200Error", "RawDecoderException", "IOException",
-           "huff_table", "unpack_plan", "raw_plan", "RawJob", "sraw_plan", "SrawJob", "arw2_plan", "Arw2Job", "nikon_plan", "NikonJob", "pana_plan", "PanaJob", "scale_plan", "ScaleJob", "dngop_plan", "DngOp", "DngOpJob", "badpix_plan", "BadPixJob", "lookup_plan", "LookupJob", "phaseone_plan", "PhaseOneJob", "PhaseOneStrip", "samsung0_plan", "SamsungV0Job", "SamsungV0Strip", "samsung1_plan", "SamsungV1Job", "samsung2_plan", "SamsungV2Job", "kodak_plan", "KodakJob", "hasselblad_plan", "HasselbladJob", "pentax_plan", "PentaxJob", "arw1_plan", "Arw1Job", "ljpeg_plan", "cr2_plan", "image_pitch",
+           "huff_table", "unpack_plan", "raw_plan", "RawJob", "sraw_plan", "SrawJob", "arw2_plan", "Arw2Job", "nikon_plan", "NikonJob", "pana_plan", "PanaJob", "scale_plan", "ScaleJob", "dngop_plan", "DngOp", "DngOpJob", "badpix_plan", "BadPixJob", "lookup_plan", "LookupJob", "phaseone_plan", "PhaseOneJob", "PhaseOneStrip", "samsung0_plan", "SamsungV0Job", "SamsungV0Strip", "samsung1_plan", "SamsungV1Job", "samsung2_plan", "SamsungV2Job", "kodak_plan", "KodakJob", "vc5_plan", "Vc5Job", "Vc5Band", "Vc5Code", "hasselblad_plan", "HasselbladJob", "pentax_plan", "PentaxJob", "arw1_plan", "Arw1Job", "ljpeg_plan", "cr2_plan", "image_pitch",
            "new_image", "UnpackJob", "LJpegScan", "Cr2Job", "HuffTable", "LSB", "MSB",
            "MSB16", "MSB32", "Comm", "comm_unique_id", "GATHER_NONE", "GATHER_ALL", "GATHER_ROOT"]

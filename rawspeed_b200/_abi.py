@@ -71,6 +71,20 @@ class KodakJob(C.Structure):
                 ("out_offset", C.c_uint64), ("out_pitch", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class Vc5Code(C.Structure):
+    _fields_ = [("size", C.c_uint32), ("bits", C.c_uint32), ("count", C.c_uint32), ("value", C.c_uint32)]
+
+
+class Vc5Band(C.Structure):
+    _fields_ = [("in_offset", C.c_uint64), ("in_size", C.c_uint32), ("param", C.c_int32)]
+
+
+class Vc5Job(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("output_bits", C.c_int32), ("phase", C.c_int32),
+                ("prescale", (C.c_uint8 * 3) * 4), ("first_band", C.c_uint32), ("out_offset", C.c_uint64),
+                ("out_pitch", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 class NikonJob(C.Structure):
     _fields_ = [("in_offset", C.c_uint64), ("in_size", C.c_uint32), ("table", C.c_uint32),
                 ("width", C.c_int32), ("height", C.c_int32), ("out_offset", C.c_uint64),
@@ -196,7 +210,7 @@ EXPORTS = [
     "rsb200_kernel_launches", "rsb200_device_sm_count", "rsb200_unpack_plan_create",
     "rsb200_raw_plan_create", "rsb200_sraw_plan_create",
     "rsb200_pentax_plan_create", "rsb200_arw1_plan_create", "rsb200_arw2_plan_create", "rsb200_nikon_plan_create",
-    "rsb200_pana_plan_create", "rsb200_phaseone_plan_create", "rsb200_samsung0_plan_create", "rsb200_samsung1_plan_create", "rsb200_samsung2_plan_create", "rsb200_kodak_plan_create", "rsb200_kodak_plan_values", "rsb200_hasselblad_plan_create", "rsb200_scale_plan_create", "rsb200_plan_bad_pixels", "rsb200_dngop_plan_create", "rsb200_badpix_plan_create", "rsb200_lookup_plan_create",
+    "rsb200_pana_plan_create", "rsb200_phaseone_plan_create", "rsb200_samsung0_plan_create", "rsb200_samsung1_plan_create", "rsb200_samsung2_plan_create", "rsb200_kodak_plan_create", "rsb200_kodak_plan_values", "rsb200_vc5_plan_create", "rsb200_hasselblad_plan_create", "rsb200_scale_plan_create", "rsb200_plan_bad_pixels", "rsb200_dngop_plan_create", "rsb200_badpix_plan_create", "rsb200_lookup_plan_create",
     "rsb200_ljpeg_plan_create", "rsb200_cr2_plan_create", "rsb200_plan_run",
     "rsb200_plan_run_host", "rsb200_plan_run_host_image", "rsb200_plan_results", "rsb200_plan_bytes",
     "rsb200_plan_launches", "rsb200_plan_kernels", "rsb200_plan_destroy",
@@ -253,6 +267,8 @@ def load():
     L.rsb200_samsung2_plan_create.argtypes = [vp, C.POINTER(SamsungV2Job), i32, C.POINTER(vp)]
     L.rsb200_kodak_plan_create.argtypes = [vp, C.POINTER(KodakJob), i32, vp, i32, C.POINTER(vp)]
     L.rsb200_kodak_plan_values.argtypes = [vp, C.POINTER(C.c_int32), i32]
+    L.rsb200_vc5_plan_create.argtypes = [vp, C.POINTER(Vc5Code), i32, C.POINTER(Vc5Job), i32,
+                                         C.POINTER(Vc5Band), i32, C.POINTER(vp)]
     L.rsb200_ljpeg_plan_create.argtypes = [vp, C.POINTER(HuffTable), i32,
                                            C.POINTER(LJpegScan), i32, C.POINTER(vp)]
     L.rsb200_cr2_plan_create.argtypes = [vp, C.POINTER(HuffTable), i32,

@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 
 from . import _abi
-from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, SamsungV2Job, KodakJob, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
+from ._abi import (Arw1Job, Arw2Job, HasselbladJob, NikonJob, PanaJob, ScaleJob, DngOp, DngOpJob, BadPixJob, LookupJob, PhaseOneJob, PhaseOneStrip, SamsungV0Job, SamsungV0Strip, SamsungV1Job, SamsungV2Job, KodakJob, Vc5Code, Vc5Job, Vc5Band, Cr2Job, HuffTable, LJpegScan, PentaxJob, RawJob, ScanResult, SrawJob, UnpackJob,  # noqa: F401
                    LSB, MSB, MSB16, MSB32)
 
 
@@ -407,6 +407,20 @@ def kodak_plan(ctx, jobs, tables=None):
         tp, nt = t.ctypes.data, t.shape[0]
     h = C.c_void_p()
     ctx.check(ctx._lib.rsb200_kodak_plan_create(ctx.h, ja, len(jobs), tp, nt, C.byref(h)))
+    return Plan(ctx, h, len(jobs))
+
+
+def vc5_plan(ctx, codebook, jobs, bands):
+    """GoPro VC-5 frames (VC5Decompressor::decode), one job per frame.  codebook: Vc5Code entries or an
+    (n, 4) array of {size, bits, count, value}; bands: the Vc5Band payloads the jobs index (40 per job,
+    channel * 10 + subband from job.first_band), as the tag walk cut them."""
+    if not (len(codebook) and isinstance(codebook[0], Vc5Code)):
+        codebook = [Vc5Code(*(int(x) for x in e)) for e in codebook]
+    ca = (Vc5Code * len(codebook))(*codebook)
+    ja = (Vc5Job * len(jobs))(*jobs)
+    ba = (Vc5Band * len(bands))(*bands)
+    h = C.c_void_p()
+    ctx.check(ctx._lib.rsb200_vc5_plan_create(ctx.h, ca, len(codebook), ja, len(jobs), ba, len(bands), C.byref(h)))
     return Plan(ctx, h, len(jobs))
 
 

@@ -15,6 +15,7 @@
 // There is no CPU fallback: forms the engine does not take raise RawDecoderException.
 #include "rawspeedconfig.h"
 #include "codes/PrefixCodeDecoder.h"
+#include "common/BayerPhase.h"
 #include "common/RawImage.h"
 #include "common/RawspeedException.h"
 #include "decoders/RawDecoderException.h"
@@ -26,6 +27,7 @@
 #include "io/IOException.h"
 
 #include "rawspeed_b200.h"
+#include "../vc5_parse.h"
 
 #include <algorithm>
 #include <cstring>
@@ -71,6 +73,83 @@ struct PlanGuard {
       rsb200_plan_destroy(p);
   }
 };
+
+// The VC-5 codebook of the integrator's reference checkout (src/external/gopro/vc5/table17.inc, on the
+// include path of this unit), in the shapes that file expects; it reaches the plan as an argument.
+struct RLV final {
+  uint_fast8_t size; // code length in bits
+  uint32_t bits;     // code word, right-justified
+  uint16_t count;    // run length
+  uint16_t value;    // run value (unsigned)
+};
+#define RLVTABLE(n)                                                                                    \
+  struct {                                                                                             \
+    const uint32_t length;                                                                             \
+    const RLV entries[n];                                                                              \
+  } constexpr
+#include "gopro/vc5/table17.inc"
+#undef RLVTABLE
+
+const std::vector<rsb200_vc5_code>& vc5_codebook() {
+  static const std::vector<rsb200_vc5_code> codes = [] {
+    std::vector<rsb200_vc5_code> c;
+    for (const RLV& e : table17.entries)
+      c.push_back(rsb200_vc5_code{e.size, e.bits, e.count, e.value});
+    return c;
+  }();
+  return codes;
+}
+
+[[noreturn]] void throw_outcome(const rsb200_vc5::Outcome& o) {
+  if (o.cls == rsb200_vc5::IOE)
+    ThrowIOE("%s", o.msg.c_str());
+  ThrowRDE("%s", o.msg.c_str());
+}
+
+// VC5Decompressor(bs, mRaw) + decode(offX, offY, width, height) of one DNG tile (the reference's
+// decompressThread<9>, AbstractDngDecompressor.cpp:161-179): the constructor's checks and the tag walk on
+// the host (vc5_parse.h), the bands and wavelets on the device, a band failure rethrown as decode() does.
+void vc5_tile(const RawImage& mRaw, const ByteStream& bs, int offX, int offY, int width, int height) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 || mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  const Optional<BayerPhase> phase = getAsBayerPhase(mRaw->cfa);
+  const uint8_t* data = bs.peekData(bs.getRemainSize());
+  const uint32_t size = static_cast<uint32_t>(bs.getRemainSize());
+  rsb200_vc5::Parsed p;
+  const rsb200_vc5::Outcome o = rsb200_vc5::parse(data, size, mRaw->dim.x, mRaw->dim.y,
+                                                  mRaw->whitePoint ? *mRaw->whitePoint : 0,
+                                                  phase ? static_cast<int>(*phase) : -1, p);
+  if (o.cls != rsb200_vc5::OK)
+    throw_outcome(o);
+  if (offX || offY || mRaw->dim != iPoint2D(width, height))
+    ThrowRDE("VC5Decompressor expects to fill the whole image, not some tile.");
+  const auto img = mRaw->getU16DataAsUncroppedArray2DRef();
+  const uint32_t pitch = static_cast<uint32_t>(img.pitch()) * 2u;
+  p.job.out_offset = 0;
+  p.job.out_pitch = pitch;
+  const std::vector<rsb200_vc5_code>& codes = vc5_codebook();
+  std::lock_guard<std::mutex> g(engine_mutex());
+  PlanGuard pg;
+  int rc = rsb200_vc5_plan_create(engine(), codes.data(), static_cast<int>(codes.size()), &p.job, 1, p.bands, 40,
+                                  &pg.p);
+  if (rc != RSB200_OK)
+    throw_status(rc, "VC5Decompressor");
+  // partial: a failed frame leaves the image as it was
+  rc = rsb200_plan_run_host_image(pg.p, data, size, reinterpret_cast<uint8_t*>(&img(0, 0)), pitch,
+                                  static_cast<uint32_t>(mRaw->dim.x) * 2u, static_cast<uint32_t>(mRaw->dim.y), 1);
+  if (rc != RSB200_OK)
+    throw_status(rc, "VC5Decompressor");
+  rsb200_scan_result res;
+  rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  if (rc != RSB200_ERR_RDE && rc != RSB200_ERR_IOE)
+    throw_status(rc, "VC5Decompressor");
+  mRaw->setError(rsb200_vc5::band_failure(res.consumed).msg);
+  std::string firstErr;
+  if (mRaw->isTooManyErrors(1, &firstErr))
+    ThrowRDE("Too many errors encountered. Giving up. First Error:\n%s", firstErr.c_str());
+}
 
 rsb200_huff_table table_of(const PrefixCodeDecoder<>& ht) {
   rsb200_huff_table t;
@@ -303,9 +382,21 @@ void AbstractDngDecompressor::decompress() const {
         mRaw->setError(err.what());
       }
     }
+  } else if (compression == 9) {
+    // VC-5 (GoPro): every tile through the device, in the reference's tile order
+    for (const auto& e : slices) {
+      try {
+        vc5_tile(mRaw, e.bs, static_cast<int>(e.offX), static_cast<int>(e.offY), static_cast<int>(e.width),
+                 static_cast<int>(e.height));
+      } catch (const RawDecoderException& err) {
+        mRaw->setError(err.what());
+      } catch (const IOException& err) {
+        mRaw->setError(err.what());
+      }
+    }
   } else {
     // uncompressed tiles go through UncompressedDecompressor::readUncompressedRaw() (below);
-    // Deflate / VC-5 / lossy JPEG tiles are outside the hot path and stay the reference's
+    // Deflate / lossy JPEG tiles are outside the hot path and stay the reference's
 #pragma omp parallel num_threads(rawspeed_get_number_of_processor_cores()) if (slices.size() > 1)
     decompressThread();
   }

@@ -403,6 +403,24 @@ int rsb200h_kodak(uint16_t* img_data, int w, int h, int cpp, int pitch, const ui
   });
 }
 
+// VC5Decompressor(bs, img, phase, codes).decode(0, 0, w, h) on an image with white level `white`;
+// codes: ncodes entries of {size, bits, count, value}
+int rsb200h_vc5(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data, uint32_t size, int white, int phase,
+                const rsb200_vc5_code* codes, int ncodes, rsb200h_err* e) {
+  return guarded(e, [&] {
+    RawImage img = makeImage(img_data, w, h, 1, pitch, true, 1, 1);
+    img->whitePoint = white;
+    try {
+      VC5Decompressor d(ByteStream(data, size), img, phase, codes, ncodes);
+      d.decode(0, 0, (unsigned)w, (unsigned)h);
+    } catch (...) {
+      copyOut(img, img_data);
+      throw;
+    }
+    copyOut(img, img_data);
+  });
+}
+
 int rsb200h_sony_arw1_decompress(uint16_t* img_data, int w, int h, int pitch, const uint8_t* data,
                                  uint32_t size, rsb200h_err* e) {
   return guarded(e, [&] {

@@ -3,6 +3,7 @@
 // reference files).  Everything here is header parsing / validation / exception
 // plumbing; every per-pixel loop of the reference is a call into
 // librawspeed_b200.so (CUDA).  There is no CPU decode path in this file.
+#include "../vc5_parse.h"
 #include "rawspeed_host.h"
 
 #include <algorithm>
@@ -995,6 +996,46 @@ void KodakDecompressor::decompress() const {
   default:
     engineCheck(rc, "rsb200_plan_results");
   }
+}
+
+// ------------------------------------------------------------------ GoPro VC-5
+VC5Decompressor::VC5Decompressor(ByteStream bs, const RawImage& img, int phase, const rsb200_vc5_code* codes_,
+                                 int ncodes)
+    : mRaw(img), mBs(bs), codes(codes_, codes_ + (ncodes > 0 ? ncodes : 0)) {
+  if (mRaw->getCpp() != 1 || mRaw->getDataType() != RawImageType::UINT16 || mRaw->getBpp() != sizeof(uint16_t))
+    ThrowRDE("Unexpected component count / data type");
+  rsb200_vc5::Parsed p;
+  const rsb200_vc5::Outcome o = rsb200_vc5::parse(mBs.begin() + mBs.getPosition(), mBs.getRemainSize(), mRaw->dim.x,
+                                                  mRaw->dim.y, mRaw->whitePoint.value_or(0), phase, p);
+  if (o.cls == rsb200_vc5::IOE)
+    ThrowIOE("%s", o.msg.c_str());
+  if (o.cls != rsb200_vc5::OK)
+    ThrowRDE("%s", o.msg.c_str());
+  job = p.job;
+  std::memcpy(bands, p.bands, sizeof bands);
+}
+
+void VC5Decompressor::decode(unsigned int offsetX, unsigned int offsetY, unsigned int width, unsigned int height) {
+  if (offsetX || offsetY || mRaw->dim.x != (int)width || mRaw->dim.y != (int)height)
+    ThrowRDE("VC5Decompressor expects to fill the whole image, not some tile.");
+  job.out_offset = 0;
+  job.out_pitch = (uint32_t)mRaw->pitch;
+  PlanGuard pg;
+  engineCheck(rsb200_vc5_plan_create(engine(), codes.data(), (int)codes.size(), &job, 1, bands, 40, &pg.p),
+              "rsb200_vc5_plan_create");
+  RawImage img = mRaw;
+  // partial: a failed frame leaves the image as it was
+  runOnImage(pg.p, mBs.begin() + mBs.getPosition(), mBs.getRemainSize(), img, /*partial=*/true);
+  rsb200_scan_result res;
+  const int rc = rsb200_plan_results(pg.p, &res, 1);
+  if (rc == RSB200_OK)
+    return;
+  if (rc != RSB200_ERR_RDE && rc != RSB200_ERR_IOE)
+    engineCheck(rc, "rsb200_plan_results");
+  mRaw->setError(rsb200_vc5::band_failure(res.consumed).msg);
+  std::string firstErr;
+  if (mRaw->isTooManyErrors(1, &firstErr))
+    ThrowRDE("Too many errors encountered. Giving up. First Error:\n%s", firstErr.c_str());
 }
 
 // ------------------------------------------------------------------ Sony ARW1

@@ -644,6 +644,28 @@ private:
   bool uncorrectedRawValues;
 };
 
+// ---------------------------------------------------------------- GoPro VC-5
+// decompressors/VC5Decompressor.h: the constructor (stream, image; its checks and the tag walk,
+// VC5Decompressor.cpp:382-618, with the reference's messages) and decode(offsetX, offsetY, width,
+// height).  Two arguments more than the reference's: the image's Bayer phase (0..3 as BayerPhase, -1
+// for a CFA that is not 2x2; this RawImage carries no CFA), and the codebook (the entries of the
+// reference's table17.inc), which goes to the plan as it is.  The bands are decoded and the wavelets
+// reconstructed on the device (vc5.cuh); a band failure goes through setError and is rethrown as
+// "Too many errors encountered. Giving up. First Error:\n..." as VC5Decompressor::decode does.
+// Images of 32 or fewer columns or rows, where the reference reads outside its bands, are refused.
+class VC5Decompressor final {
+public:
+  VC5Decompressor(ByteStream bs, const RawImage& img, int phase, const rsb200_vc5_code* codes, int ncodes);
+  void decode(unsigned int offsetX, unsigned int offsetY, unsigned int width, unsigned int height);
+
+private:
+  RawImage mRaw;
+  ByteStream mBs;
+  std::vector<rsb200_vc5_code> codes;
+  rsb200_vc5_job job;
+  rsb200_vc5_band bands[40];
+};
+
 // ---------------------------------------------------------------- Sony ARW1
 // decompressors/SonyArw1Decompressor.h: same constructor (image; its checks,
 // SonyArw1Decompressor.cpp:39-50) and decompress(ByteStream).  The whole decode runs

@@ -33,6 +33,7 @@
 #include "samsung1.cuh"
 #include "samsung2.cuh"
 #include "kodak.cuh"
+#include "vc5.cuh"
 #include "unpack.cuh"
 
 #include <algorithm>
@@ -45,6 +46,8 @@
 #include <new>
 #include <string>
 #include <chrono>
+#include <cmath>
+#include <functional>
 #include <thread>
 #include <variant>
 #include <vector>
@@ -405,6 +408,23 @@ struct KodakPlan {
   DevPtr<int32_t> d_kd_values;
 };
 
+// GoPro VC-5 (vc5.cuh)
+struct Vc5Plan {
+  DevPtr<uint32_t> d_code;      // multi-level decode table
+  DevPtr<Vc5FrameDev> d_frames;
+  DevPtr<Vc5BandDev> d_bands;   // 40 per frame
+  DevPtr<uint32_t> d_seg_band;  // per segment: its band
+  DevPtr<uint2> d_map;          // two ping-pong buffers of nsegs * VC5_CAND
+  DevPtr<unsigned long long> d_err;  // per band: first failure, bit position << 3 | code
+  DevPtr<int16_t> d_coef;       // bands and the level-3 / level-2 reconstructions
+  DevPtr<uint16_t> d_luts;      // log tables of output bits 1..16
+  uint64_t ncoef = 0;
+  uint32_t nsegs = 0, rounds = 0;
+  uint32_t max_low = 0, max_rec[2] = {0, 0}, max_quads = 0;  // grid sizes
+  DevPtr<uint2> d_job_res;
+  PinnedPtr<uint2> h_job_res;
+};
+
 // Sony ARW2
 struct Arw2Plan {
   DevPtr<Arw2JobDev> d_arw2_jobs;
@@ -511,7 +531,7 @@ struct rsb200_plan {
   cudaStream_t last_stream = nullptr;
   bool ran = false;
   std::variant<UnpackPlan, LjpegPlan, RawFormPlan, SrawPlan, Arw2Plan, PanaPlan, PhaseOnePlan, ScalePlan, DngOpPlan,
-               BadPixPlan, LookupPlan, HasselbladPlan, SamsungV0Plan, SamsungV2Plan, KodakPlan>
+               BadPixPlan, LookupPlan, HasselbladPlan, SamsungV0Plan, SamsungV2Plan, KodakPlan, Vc5Plan>
       state;
 };
 
@@ -2094,6 +2114,115 @@ extern "C" int rsb200_kodak_plan_values(rsb200_plan* p, int32_t* values, int n) 
   if (take > 0)
     CUDA_TRY(ctx, cudaMemcpy(values, s->d_kd_values.get(), sizeof(int32_t) * (size_t)take, cudaMemcpyDeviceToHost));
   return RSB200_OK;
+}
+
+// ------------------------------------------------------------------
+// GoPro VC-5: band payloads cut into segments, exact entries by a scan of candidate walks (vc5.cuh)
+// ------------------------------------------------------------------
+extern "C" int rsb200_vc5_plan_create(rsb200_ctx* ctx, const rsb200_vc5_code* codes, int ncodes,
+                                      const rsb200_vc5_job* jobs, int njobs, const rsb200_vc5_band* bands, int nbands,
+                                      rsb200_plan** out) {
+  if (!ctx || !codes || !jobs || njobs <= 0 || njobs > 16383 || !bands || nbands <= 0 || !out)
+    return set_err(ctx, RSB200_ERR_ARG, "vc5_plan_create: bad arguments");
+  std::vector<uint32_t> code;
+  if (!vc5_build_code(codes, ncodes, code))
+    return set_err(ctx, RSB200_ERR_ARG, "vc5_plan_create: the codebook is not a complete prefix code within limits");
+  CUDA_TRY(ctx, cudaSetDevice(ctx->device));
+  PlanHolder holder = new_plan(ctx);
+  if (!holder)
+    return RSB200_ERR_CUDA;
+  rsb200_plan* p = holder.get();
+  Vc5Plan& s = p->state.emplace<Vc5Plan>();
+  p->nunits = njobs;
+  Vc5Layout L;
+  const char* why = nullptr;
+  const int bad = vc5_layout(jobs, njobs, bands, nbands, L, &why);
+  if (bad >= 0)
+    return set_err(ctx, RSB200_ERR_ARG, "vc5 job %d: %s", bad, why);
+  for (int i = 0; i < njobs; ++i) {
+    const rsb200_vc5_job& j = jobs[i];
+    for (int b = 0; b < 40; ++b) {
+      const rsb200_vc5_band& band = bands[j.first_band + (uint32_t)b];
+      p->in_bytes += band.in_size;
+      p->need_in = std::max<uint64_t>(p->need_in, sat_add(band.in_offset, band.in_size));
+    }
+    p->out_bytes += (uint64_t)j.width * j.height * 2;
+    p->pixels += (uint64_t)j.width * j.height;
+    p->need_out = std::max<uint64_t>(p->need_out,
+                                     sat_add(j.out_offset, ((uint64_t)j.height - 1) * j.out_pitch + 2ull * j.width));
+  }
+  s.ncoef = L.ncoef;
+  s.nsegs = (uint32_t)L.seg_band.size();
+  s.rounds = L.rounds;
+  s.max_low = L.max_low, s.max_rec[0] = L.max_rec[0], s.max_rec[1] = L.max_rec[1], s.max_quads = L.max_quads;
+  const std::vector<uint16_t> luts = vc5_luts();
+  cudaError_t e = cudaSuccess;
+  dev_upload(e, s.d_code, code.data(), sizeof(uint32_t) * code.size());
+  dev_upload(e, s.d_frames, L.frames.data(), sizeof(Vc5FrameDev) * L.frames.size());
+  dev_upload(e, s.d_bands, L.bands.data(), sizeof(Vc5BandDev) * L.bands.size());
+  dev_upload(e, s.d_seg_band, L.seg_band.data(), sizeof(uint32_t) * L.seg_band.size());
+  dev_upload(e, s.d_luts, luts.data(), sizeof(uint16_t) * luts.size());
+  dev_alloc(e, s.d_map, sizeof(uint2) * 2 * (size_t)s.nsegs * VC5_CAND);
+  dev_alloc(e, s.d_err, sizeof(unsigned long long) * L.bands.size());
+  dev_alloc(e, s.d_coef, sizeof(int16_t) * L.ncoef);
+  dev_alloc(e, s.d_job_res, sizeof(uint2) * (size_t)njobs);
+  host_alloc(e, s.h_job_res, sizeof(uint2) * (size_t)njobs);
+  if (e != cudaSuccess)
+    return set_err(ctx, RSB200_ERR_CUDA, "vc5 plan allocation failed: %s", cudaGetErrorString(e));
+  p->launches_per_run = 7 + (int)s.rounds;
+  *out = holder.release();
+  return RSB200_OK;
+}
+
+static int run(const rsb200_plan* p, const Vc5Plan& s, const uint8_t* in, uint64_t, uint8_t* outp, cudaStream_t st) {
+  const uint32_t nf = (uint32_t)p->nunits;
+  auto blocks = [](uint64_t n) { return (uint32_t)std::max<uint64_t>(1, (n + VC5_NT - 1) / VC5_NT); };
+  const Vc5FrameDev* fr = s.d_frames.get();
+  const Vc5BandDev* bd = s.d_bands.get();
+  int16_t* coef = s.d_coef.get();
+  CUDA_TRY(p->ctx, cudaMemsetAsync(s.d_err.get(), 0xFF, sizeof(unsigned long long) * 40 * nf, st));
+  CUDA_TRY(p->ctx, cudaMemsetAsync(coef, 0, sizeof(int16_t) * s.ncoef, st));
+  vc5_lowpass_kernel<<<dim3(blocks(s.max_low), 4 * nf), VC5_NT, 0, st>>>(in, bd, coef);
+  const uint32_t gm = blocks((uint64_t)s.nsegs * VC5_CAND);
+  uint2* a = s.d_map.get();
+  uint2* b = a + (size_t)s.nsegs * VC5_CAND;
+  vc5_walk_kernel<<<gm, VC5_NT, 0, st>>>(in, bd, s.d_seg_band.get(), s.nsegs, s.d_code.get(), a);
+  for (uint32_t r = 0; r < s.rounds; ++r) {
+    vc5_scan_kernel<<<gm, VC5_NT, 0, st>>>(bd, s.d_seg_band.get(), s.nsegs, r, a, b);
+    std::swap(a, b);
+  }
+  vc5_store_kernel<<<blocks(s.nsegs), VC5_NT, 0, st>>>(in, bd, s.d_seg_band.get(), s.nsegs, s.d_code.get(), a,
+                                                       s.d_err.get(), coef);
+  vc5_result_kernel<<<blocks(nf), VC5_NT, 0, st>>>(fr, nf, bd, s.d_err.get(), s.d_job_res.get());
+  vc5_recon_kernel<<<dim3(blocks(s.max_rec[0]), 4 * nf), VC5_NT, 0, st>>>(fr, bd, 0, coef);
+  vc5_recon_kernel<<<dim3(blocks(s.max_rec[1]), 4 * nf), VC5_NT, 0, st>>>(fr, bd, 1, coef);
+  vc5_final_kernel<<<dim3(blocks(s.max_quads), nf), VC5_NT, 0, st>>>(fr, bd, coef, s.d_luts.get(),
+                                                                       s.d_job_res.get(), outp);
+  CUDA_TRY(p->ctx, cudaGetLastError());
+  p->ctx->launches += (uint64_t)p->launches_per_run;
+  return RSB200_OK;
+}
+
+static int results(const rsb200_plan* p, Vc5Plan& s, rsb200_scan_result* out, int n) {
+  // VC5Decompressor.cpp:683-742, :849-873; BitStreamer.h:58-59, :125-127
+  static const char* const text[7] = {"",
+                                      "Impossible RLV value given current quantum",
+                                      "Got EndOfBand marker while looking for next pixel",
+                                      "Not all pixels consumed?",
+                                      "EndOfBand marker not found",
+                                      "Bit stream size is smaller than MaxProcessBytes",
+                                      "Buffer overflow read in BitStreamer"};
+  return report_jobs(
+      p, s.d_job_res, s.h_job_res, out, n, [&](int i) { return rsb200_scan_result{s.h_job_res[i].x, s.h_job_res[i].y}; },
+      [&](int i, const rsb200_scan_result& r) {
+        set_err(p->ctx, (int)r.status, "job %d: Too many errors encountered. Giving up. First Error:\n%s (channel %u, subband %u)",
+                i, text[std::min<uint32_t>(r.consumed >> 28, 6u)], (r.consumed >> 4) & 15u, r.consumed & 15u);
+      });
+}
+
+static const char* kernels(const rsb200_plan*, const Vc5Plan&) {
+  return "vc5_lowpass_kernel + vc5_walk_kernel + vc5_scan_kernel + vc5_store_kernel + vc5_result_kernel + "
+         "vc5_recon_kernel + vc5_final_kernel";
 }
 
 // ------------------------------------------------------------------

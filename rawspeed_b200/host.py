@@ -28,7 +28,7 @@ class _Huff(C.Structure):
 
 EXPORTS = ["rsb200h_unpack", "rsb200h_ljpeg_decompress", "rsb200h_ljpeg_decode",
            "rsb200h_dng_decompress", "rsb200h_cr2_decompress", "rsb200h_cr2_ljpeg_decode",
-           "rsb200h_huff_check", "rsb200h_unpack_form", "rsb200h_pentax_decompress", "rsb200h_sony_arw1_decompress", "rsb200h_samsung_v0", "rsb200h_samsung_v1", "rsb200h_samsung_v2", "rsb200h_kodak",
+           "rsb200h_huff_check", "rsb200h_unpack_form", "rsb200h_pentax_decompress", "rsb200h_sony_arw1_decompress", "rsb200h_samsung_v0", "rsb200h_samsung_v1", "rsb200h_samsung_v2", "rsb200h_kodak", "rsb200h_vc5",
            "rsb200h_sraw_interpolate", "rsb200h_nikon_decompress", "rsb200h_sony_arw2",
            "rsb200h_panasonic", "rsb200h_phaseone", "rsb200h_scale_black_white",
            "rsb200h_panasonic_v4", "rsb200h_dng_opcodes", "rsb200h_dngop_lower",
@@ -241,6 +241,21 @@ def kodak(img, w, data, bps=12, uncorrected=False, curve=None, dither=False, cpp
     e.check(L.rsb200h_kodak(C.c_void_p(img.ctypes.data), w, img.shape[0], cpp, img.shape[1] * 2, p, C.c_uint32(n),
                             bps, int(uncorrected), None if cv is None else C.c_void_p(cv.ctypes.data),
                             0 if cv is None else cv.size, int(dither), C.byref(e)))
+    return img
+
+
+def vc5(img, w, data, white, phase, codes):
+    """VC5Decompressor(data, img, phase, codes).decode(0, 0, w, h) via the host mirror, on an image of white
+    level `white` and Bayer phase `phase` (0..3, -1: not a 2x2 CFA); img is (h, pitch) uint16; codes: the
+    codebook as an (n, 4) array of {size, bits, count, value}."""
+    p, n = _u8(data)
+    e = _Err()
+    L = lib()
+    L.rsb200h_vc5.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_uint32, C.c_int, C.c_int,
+                              C.c_void_p, C.c_int, C.POINTER(_Err)]
+    cb = np.ascontiguousarray(codes, np.uint32).reshape(-1, 4)
+    e.check(L.rsb200h_vc5(C.c_void_p(img.ctypes.data), w, img.shape[0], img.shape[1] * 2, p, C.c_uint32(n), white,
+                          phase, C.c_void_p(cb.ctypes.data), cb.shape[0], C.byref(e)))
     return img
 
 
